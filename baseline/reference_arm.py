@@ -1,4 +1,4 @@
-"""Reference arm of ``bench.py``: the UNMODIFIED reference (installed in ``baseline/_ref`` from a copy of
+"""Reference arm of ``bench.py``: the UNMODIFIED reference (installed in ``oracle/_ref`` from a copy of
 ``/root/reference`` plus a packaging shim) driven through its own public API – ``builder.parser_server`` /
 ``builder.parser_clients`` / ``experiment.ExperimentStage._process_one_round`` – on the same synthetic workload.
 
@@ -23,7 +23,7 @@ import time
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 _T_IMPORT = time.perf_counter()          # ~process start: bench.py imports this module first thing in the arm
-REF = os.path.join(HERE, "_ref")
+REF = os.path.join(os.path.dirname(HERE), "oracle", "_ref")
 
 
 def _unavailable(why: str) -> dict:
@@ -80,7 +80,7 @@ def run_reference_arm(a, build_config, cleanup_payloads, metric, ClockSampler, b
     rank = int(os.environ.get("RANK", 0))
     world = int(os.environ.get("WORLD_SIZE", 1))
     if not os.path.isdir(os.path.join(REF, "methods")):
-        return _unavailable("baseline/_ref is missing (pip install --target of the reference copy was not run)")
+        return _unavailable("oracle/_ref is missing (the reference oracle was not built: oracle/install_reference.sh)")
     if world > 1:
         import torch.distributed as dist
         dist.init_process_group("gloo")

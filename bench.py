@@ -9,7 +9,7 @@ FedAvg aggregation into the server model, with the reference's checkpoint files 
 ``e2e``   = the same metric measured by wall clock around the public API (``ExperimentStage`` rounds): every batch is
 copied host->device from pinned memory and every epoch's loss/accuracy is read back.
 
-``--impl reference`` runs the UNMODIFIED reference installed in ``baseline/_ref`` through its own builder /
+``--impl reference`` runs the UNMODIFIED reference installed in ``oracle/_ref`` through its own builder /
 ``ExperimentStage._process_one_round`` on the same synthetic workload. ``--impl nccl`` runs this engine with the
 collectives expressed as plain ``torch.distributed`` (NCCL) calls – the "baseline, not the product" harness.
 """
@@ -90,11 +90,14 @@ def parse_args():
                          "the same engine with fp32 activations / weights on the library kernels (the precision-matched "
                          "arm for convergence comparisons with the fp32 reference; not the headline)")
     ap.add_argument("--cpu-debug", action="store_true", help="tiny CPU run to exercise the harness")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed rounds, write what the last timed round computed (server and client "
+                         "parameters, per-client training loss / accuracy) as DIR/<name>.npy")
     return ap.parse_args()
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -195,7 +198,7 @@ def bench_config(a, impl: str, parallelism: str) -> dict:
             if a.method.startswith("fedstil") else
             "one communication round of the reference's loop (experiment.py:183-243): dispatch + local train of all "
             "online clients (full backbone in train mode) + upload + aggregate",
-            "l2": "inputs larger than L2 (per-round working set >> 126 MB: 8 x 400 MB client state + images)"}
+            "l2": "inputs larger than L2 (per-round working set >> 50 MB: 8 x 400 MB client state + images)"}
 
 
 def convergence_block(records: dict, rounds: int) -> dict:
@@ -215,6 +218,37 @@ def convergence_block(records: dict, rounds: int) -> dict:
             loss.append(round(sum(l_) / len(l_), 4))
     return {"rounds": len(acc), "tr_acc_pct": acc, "tr_loss": loss,
             "final_tr_acc_pct": acc[-1] if acc else None, "final_tr_loss": loss[-1] if loss else None}
+
+
+DUMP_SAMPLE = 1 << 20          # elements kept per parameter arena by --dump-outputs (4 MB each in float32)
+
+
+def dump_outputs(out_dir: str, server, clients, records: dict, rnd: int) -> None:
+    """What a round hands its caller: the aggregated server parameters, every client's parameters and the per-client
+    training loss / accuracy of round ``rnd``. An arena larger than ``DUMP_SAMPLE`` elements is reduced to a fixed,
+    seeded sample of its elements (the same indices for the same arena size), so the files stay within 64 MB."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+
+    def arena(name, model):
+        flat = model.arena.master.detach().reshape(-1)
+        if flat.numel() > DUMP_SAMPLE:
+            g = torch.Generator().manual_seed(0)
+            idx = torch.randint(0, flat.numel(), (DUMP_SAMPLE,), generator=g).to(flat.device)
+            flat = flat[idx]
+        np.save(os.path.join(out_dir, f"{name}.npy"), flat.float().cpu().numpy())
+
+    arena("server_params", server.model)
+    loss, acc = [], []
+    for i, c in enumerate(clients):
+        arena(f"client{i}_params", c.model)
+        per_round = (records.get("data", {}).get(c.client_name) or {})
+        tasks = per_round.get(rnd) or per_round.get(str(rnd)) or {}
+        loss.append([float(t["tr_loss"]) for t in tasks.values() if "tr_loss" in t])
+        acc.append([float(t["tr_acc"]) for t in tasks.values() if "tr_acc" in t])
+    np.save(os.path.join(out_dir, "train_loss.npy"), np.asarray(loss, dtype=np.float64))
+    np.save(os.path.join(out_dir, "train_acc.npy"), np.asarray(acc, dtype=np.float64))
 
 
 def cleanup_payloads(ckpt_dir: str) -> None:
@@ -321,6 +355,8 @@ def run_flpr(a, impl: str) -> dict:
         launches = native.launches() - launches0
         h2d1 = sum(getattr(t["tr_loader"], "h2d_bytes", 0) for c in clients for t in c.task_pipeline._cache.values())
         clocks = sampler.stop() if sampler else None
+        if a.dump_outputs and rank == 0:
+            dump_outputs(a.dump_outputs, server, clients, log.records, r)
         after_round()
 
         # ---- end-to-end region: K more rounds by wall clock through the public API ---------------------------------

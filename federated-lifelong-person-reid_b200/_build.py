@@ -1,4 +1,4 @@
-"""In-tree build of the sm_100a native library (``lib/libflpr_b200.so``).
+"""In-tree build of the sm_90a native library (``lib/libflpr_b200.so``).
 
 Plain ``nvcc`` (no torch C++ headers: the kernels expose a C ABI and are driven through ``ctypes``), so a full
 rebuild takes well under a minute and the resulting ``.so`` travels with the repo snapshot to the GPU box.
@@ -19,11 +19,11 @@ OBJ_DIR = os.path.join(PKG_DIR, "build")
 LIB_PATH = os.path.join(LIB_DIR, "libflpr_b200.so")
 STAMP = os.path.join(LIB_DIR, "build.stamp")
 
-CUDA_SOURCES = ["gemm_tcgen05.cu", "fedcomm.cu", "fused_ops.cu", "loss_ops.cu", "layer_ops.cu"]
+CUDA_SOURCES = ["gemm_wgmma.cu", "fedcomm.cu", "fused_ops.cu", "loss_ops.cu", "layer_ops.cu"]
 CXX_SOURCES = ["runtime.cpp"]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -56,7 +56,7 @@ def is_current() -> bool:
 
 
 def build(force: bool = False, verbose: bool = True) -> str:
-    """Compile every native source for sm_100a and link ``libflpr_b200.so``. Returns the library path."""
+    """Compile every native source for sm_90a and link ``libflpr_b200.so``. Returns the library path."""
     if not force and is_current():
         return LIB_PATH
     os.makedirs(LIB_DIR, exist_ok=True)
@@ -69,7 +69,7 @@ def build(force: bool = False, verbose: bool = True) -> str:
         cmd = [nvcc, *NVCC_FLAGS, "-c", os.path.join(CSRC, src), "-o", obj]
         if src.endswith(".cpp"):
             cmd = [nvcc, "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-x", "cu", "-gencode",
-                   "arch=compute_100a,code=sm_100a", "-c", os.path.join(CSRC, src), "-o", obj]
+                   "arch=compute_90a,code=sm_90a", "-c", os.path.join(CSRC, src), "-o", obj]
         if verbose:
             print("[flpr_b200 build]", " ".join(cmd), flush=True)
         r = subprocess.run(cmd, capture_output=True, text=True)
@@ -79,7 +79,7 @@ def build(force: bool = False, verbose: bool = True) -> str:
 
     with ThreadPoolExecutor(max_workers=min(4, len(sources))) as pool:
         objs = list(pool.map(compile_one, sources))
-    link = [nvcc, "-shared", "-o", LIB_PATH, *objs, "-gencode", "arch=compute_100a,code=sm_100a", "-lpthread"]
+    link = [nvcc, "-shared", "-o", LIB_PATH, *objs, "-gencode", "arch=compute_90a,code=sm_90a", "-lpthread"]
     if verbose:
         print("[flpr_b200 build]", " ".join(link), flush=True)
     r = subprocess.run(link, capture_output=True, text=True)

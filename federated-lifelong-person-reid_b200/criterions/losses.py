@@ -3,7 +3,7 @@
 * :class:`CrossEntropyLabelSmooth` – ``criterions/cross_entropy.py`` (the only loss any shipped config uses); on
   CUDA it is one fused kernel (log-softmax + smoothing + gradient + top-1 count) instead of a CPU one-hot scatter.
 * :class:`TripletLoss` – ``criterions/triplet_loss.py`` (euclid / cosine distance matrix, hard or softmax-weighted
-  mining, margin-ranking or soft-margin); the distance matrix runs on the tcgen05 GEMM for CUDA inputs.
+  mining, margin-ranking or soft-margin); the distance matrix runs on the wgmma GEMM for CUDA inputs.
 * :class:`DistillKL` – ``criterions/kd_loss.py`` (dead code in the reference: never registered). Registered here
   as ``kd_loss`` because BASELINE.json names a CE+triplet+KD configuration.
 """
@@ -81,7 +81,7 @@ class TripletLoss(CriterionModule):
         return e / (e.sum(dim=1, keepdim=True) + 1e-6)
 
     def mine(self, feature: torch.Tensor, target: torch.Tensor):
-        """``(dist_ap, dist_an)``: on CUDA the Gram matrix runs on the tcgen05 GEMM (forward and both gradients) with
+        """``(dist_ap, dist_an)``: on CUDA the Gram matrix runs on the wgmma GEMM (forward and both gradients) with
         the distance / mask / mining arithmetic fused in one kernel per direction (``csrc/loss_ops.cu``)."""
         if fops.mined_distances_supported(feature) and getattr(self, "fused", True):
             x = F.normalize(feature.float(), p=2, dim=1) if self.norm_feat else feature

@@ -43,6 +43,7 @@ struct OptArgs {
   const float* G;       // FedSTIL global weight (nullable)
   __nv_bfloat16* p_bf16;  // compute copy (nullable)
   float* stats;         // [0] += sum(Q p^2 - 2 R p), [1] += sum |p - G|   (nullable)
+  float* stats_part;    // per-block partials of the two sums, folded into stats in block order by opt_stats_kernel
   size_t n;
   float lr, beta1, beta2, eps, wd, bc1, bc2_sqrt;
   float lam2;           // penalty strength (gradient gets 2*lam2*(Q p - R))
@@ -176,10 +177,23 @@ __global__ void __launch_bounds__(256) fused_opt_kernel(const OptArgs a) {
     const float s0 = block_sum(pen, sh);
     const float s1 = block_sum(l1, sh);
     if (threadIdx.x == 0) {
-      if (a.R) atomicAdd(a.stats + 0, s0);
-      if (a.G) atomicAdd(a.stats + 1, s1);
+      a.stats_part[2 * blockIdx.x] = s0;
+      a.stats_part[2 * blockIdx.x + 1] = s1;
     }
   }
+}
+
+// stats[0] += sum of the blocks' penalty partials (when R is given), stats[1] += L1 partials (when G is given), in
+// block order: the reported penalty is reproducible.
+__global__ void opt_stats_kernel(const float* part, float* stats, int blocks, int has_r, int has_g) {
+  if (threadIdx.x != 0) return;
+  float s0 = 0.f, s1 = 0.f;
+  for (int b = 0; b < blocks; ++b) {
+    s0 += part[2 * b];
+    s1 += part[2 * b + 1];
+  }
+  if (has_r) stats[0] += s0;
+  if (has_g) stats[1] += s1;
 }
 
 // F += scale * g^2 (mode 0) or scale * |g| (mode 1)
@@ -232,10 +246,10 @@ __global__ void __launch_bounds__(256) compose_kernel(const float* G, const floa
 
 // ----------------------------------------------------------------------------- label-smoothing CE
 // One block per sample. logits: [B, C] (bf16 or fp32, row stride ld). dlogits same layout (bf16 or fp32).
-// stats[0] += loss_row / B ; stats[1] += (argmax == target)
+// row_part[2 row] = loss_row / B, row_part[2 row + 1] = (argmax == target); ce_stats_kernel folds them into stats.
 template <typename TIn, typename TOut>
 __global__ void __launch_bounds__(256) ce_ls_kernel(const TIn* logits, const long long* target, TOut* dlogits,
-                                                    float* stats, int B, int C, long long ld, float eps,
+                                                    float* row_part, int B, int C, long long ld, float eps,
                                                     float grad_scale) {
   __shared__ float sh[8];
   __shared__ float s_bcast[2];
@@ -284,8 +298,8 @@ __global__ void __launch_bounds__(256) ce_ls_kernel(const TIn* logits, const lon
     const float zy = static_cast<float>(z[y]);
     // -(1-eps)*(z_y - lse) - eps/C * (sum z - C*lse)
     const float loss = -(1.f - eps) * (zy - lse) - (eps / C) * (tot_z - C * lse);
-    atomicAdd(stats + 0, loss / B);
-    if (s_arg == (int)y) atomicAdd(stats + 1, 1.f);
+    row_part[2 * row] = loss / B;
+    row_part[2 * row + 1] = s_arg == (int)y ? 1.f : 0.f;
   }
   if (dlogits != nullptr) {
     TOut* d = dlogits + (long long)row * ld;
@@ -296,6 +310,18 @@ __global__ void __launch_bounds__(256) ce_ls_kernel(const TIn* logits, const lon
       d[c] = static_cast<TOut>((pr - t) * grad_scale);
     }
   }
+}
+
+// stats[0] += sum of the rows' losses, stats[1] += hits, summed in row order (a reproducible loss value).
+__global__ void ce_stats_kernel(const float* row_part, float* stats, int B) {
+  if (threadIdx.x != 0) return;
+  float loss = 0.f, hits = 0.f;
+  for (int r = 0; r < B; ++r) {
+    loss += row_part[2 * r];
+    hits += row_part[2 * r + 1];
+  }
+  stats[0] += loss;
+  stats[1] += hits;
 }
 
 // ----------------------------------------------------------------------------- batch norm (NHWC, [M, C] bf16)
@@ -965,25 +991,24 @@ __global__ void __launch_bounds__(64) window_attn_fwd_kernel(const T* qkv, const
 // Backward: recompute P, then dV = P^T dO, dP = dO V^T, dS = P (.) (dP - rowsum(dP (.) P)), dQ = scale dS K,
 // dK = scale dS^T Q, dBias += dS (atomic over the images that share a window index).
 
-// ----------------------------------------------------------------------------- Swin window attention on tcgen05
+// ----------------------------------------------------------------------------- Swin window attention on wgmma
 // Forward only (the frozen stages never need a gradient; the trainable stage's backward keeps the kernel above).
-// A persistent CTA of 128 threads walks (window, head) pairs. Per pair:
-//   * Q [N x 32], K [N x 32] are copied into 128B-swizzled K-major operand tiles (rows = tokens padded to 128 / 64, the
+// A persistent CTA of one warpgroup (128 threads) walks (window, head) pairs. Per pair:
+//   * Q [N x 32], K [N x 32] are copied into 128B-swizzled K-major operand tiles (rows = tokens padded to 64, the
 //     K extent padded 32 -> 64 with zeros written once), V is TRANSPOSED on the way in (Vt [32 x N], K extent = keys);
-//   * S = Q K^T: two tcgen05.mma (M 128, N 64, K 16) into 64 TMEM columns;
-//   * softmax: thread = row (tcgen05.ld 32x32b gives every thread its whole 64-column score row, so max / sum need no
-//     shuffles), + relative-position bias (+ shift mask), exp2 with the scale folded in; P (bf16, un-normalised) is
-//     written back as the next A operand, 1 / sum stays in a register;
-//   * O = P V: four tcgen05.mma (M 128, N 32, K 16) into 32 more TMEM columns; epilogue scales by 1 / sum and stores
-//     the 64-byte output row.
+//   * S = Q K^T: two wgmma m64n64k16 into 32 fp32 registers per thread;
+//   * softmax on the accumulator fragment: each row lives in the 4 lanes of a quad (two rows per thread), so max / sum
+//     take two shuffles; + relative-position bias (+ shift mask), exp2 with the scale folded in; P (bf16,
+//     un-normalised) is written back as the next A operand, 1 / sum stays in a register;
+//   * O = P V: four wgmma m64n32k16; the epilogue scales by 1 / sum and stores bf16 pairs.
 // Swin: N = 49 (or 16), D = 32 for every model size. Reference: models/swin_transformer.py:255-286.
 constexpr int WA_THREADS = 128;
-constexpr int WA_SQ = 0;                       // 128 rows x 128 B
-constexpr int WA_SK = 128 * 128;               //  64 rows x 128 B
-constexpr int WA_SVT = WA_SK + 64 * 128;       //  32 rows x 128 B
-constexpr int WA_SP = WA_SVT + 32 * 128;       // 128 rows x 128 B   (WA_SVT is 4 KB: WA_SP stays 1024-aligned)
-constexpr int WA_BAR = WA_SP + 128 * 128;
-constexpr int WA_SMEM = WA_BAR + 64 + 1024;
+constexpr int WA_SQ = 0;                       // 64 rows x 128 B
+constexpr int WA_SK = 64 * 128;                // 64 rows x 128 B
+constexpr int WA_SVT = WA_SK + 64 * 128;       // 32 rows x 128 B
+constexpr int WA_SP = WA_SVT + 32 * 128;       // 64 rows x 128 B   (WA_SVT is 4 KB: WA_SP stays 1024-aligned)
+constexpr int WA_END = WA_SP + 64 * 128;
+constexpr int WA_SMEM = WA_END + 1024;
 
 // byte offset of 16-byte chunk `c` (0..7) of row `r` in a K-major SWIZZLE_128B tile (8-row x 128 B atoms)
 __device__ __forceinline__ uint32_t wa_swz(int r, int c) { return (uint32_t)(r * 128 + ((c ^ (r & 7)) << 4)); }
@@ -993,31 +1018,17 @@ window_attn_fwd_tc_kernel(const __nv_bfloat16* qkv, const float* bias, __nv_bflo
                           float scale, int total_pairs) {
   extern __shared__ uint8_t wa_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(wa_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bar = reinterpret_cast<uint64_t*>(smem + WA_BAR);
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(smem + WA_BAR + 16);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   constexpr int D = 32;
 
-  for (int i = tid; i < WA_BAR / 16; i += WA_THREADS) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
-  if (tid == 0) {
-    mbar_init(bar, 1);
-    fence_mbar_init();
-  }
-  if (warp == 0) {
-    tmem_alloc(tmem_ptr, 128);
-    tmem_relinquish();
-  }
-  tc_fence_before();
+  for (int i = tid; i < WA_END / 16; i += WA_THREADS) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_ptr;
   const uint32_t sQ = smem_u32(smem + WA_SQ), sK = smem_u32(smem + WA_SK), sVt = smem_u32(smem + WA_SVT),
                  sP = smem_u32(smem + WA_SP);
-  constexpr uint32_t idesc_s = make_idesc_bf16(128, 64, 0, 0);
-  constexpr uint32_t idesc_o = make_idesc_bf16(128, 32, 0, 0);
   const size_t row_stride = (size_t)3 * H * D;
   const float sl2 = scale * 1.4426950408889634f;            // exp(x) = exp2(x * log2 e)
-  uint32_t phase = 0;
+  // accumulator fragment of this thread: rows r0 and r0 + 8, columns 8j + c0 + {0, 1}
+  const int r0 = warp * 16 + (lane >> 2), c0 = 2 * (lane & 3);
 
   for (int p = blockIdx.x; p < total_pairs; p += gridDim.x) {
     const int bw = p / H, h = p - bw * H;
@@ -1038,99 +1049,87 @@ window_attn_fwd_tc_kernel(const __nv_bfloat16* qkv, const float* bias, __nv_bflo
         *reinterpret_cast<__nv_bfloat16*>(smem + WA_SVT + wa_swz(d, r >> 3) + (r & 7) * 2) = ve[e];
       }
     }
-    fence_proxy_async();                                     // generic-proxy smem writes -> visible to tcgen05.mma
-    tc_fence_before();
+    fence_proxy_async();                                     // generic-proxy smem writes -> visible to wgmma
     __syncthreads();
-    tc_fence_after();
-    if (tid == 0) {
+    float s[32];
 #pragma unroll
-      for (int k = 0; k < 2; ++k)                            // D = 32 -> two K = 16 steps (the padded half is zero)
-        umma_f16(tmem, make_smem_desc_sw128(sQ + k * 32, 16, 1024), make_smem_desc_sw128(sK + k * 32, 16, 1024),
-                 idesc_s, k != 0);
-      umma_commit(bar);
-    }
-    mbar_wait(bar, phase);
-    phase ^= 1;
-    tc_fence_after();
-    // ---- softmax: thread = row
-    const int r = tid;
-    float inv = 0.f;
-    if (warp < 2) {                                          // rows 0..63 (N <= 64); warp-uniform TMEM loads
-      uint32_t s0[32], s1[32];
-      const uint32_t tb = tmem + (uint32_t(warp * 32) << 16);
-      tmem_ld_32x32b_x32(tb, s0);
-      tmem_ld_32x32b_x32(tb + 32, s1);
-      tmem_ld_wait();
-      if (r < N) {
-        const float* brow = bias + (((size_t)(bw % nWb) * H + h) * N + r) * N;
-        float v[64];
-        float mx = -3.0e38f;
+    for (int j = 0; j < 32; ++j) s[j] = 0.f;
+    wgmma_fence();
 #pragma unroll
-        for (int j = 0; j < 64; ++j) {
-          const float sc = __uint_as_float(j < 32 ? s0[j & 31] : s1[j & 31]);
-          const float x = (j < N) ? fmaf(sc, sl2, brow[j] * 1.4426950408889634f) : -3.0e38f;
-          v[j] = x;
+    for (int k = 0; k < 2; ++k)                              // D = 32 -> two K = 16 steps (the padded half is unused)
+      wgmma_m64n64k16<0, 0>(s, make_smem_desc_sw128(sQ + k * 32, 16, 1024),
+                            make_smem_desc_sw128(sK + k * 32, 16, 1024), 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+#pragma unroll
+    for (int j = 0; j < 32; ++j) reg_fence(s[j]);
+    // ---- softmax on the fragment: half 0 = row r0, half 1 = row r0 + 8
+    float inv[2];
+#pragma unroll
+    for (int hf = 0; hf < 2; ++hf) {
+      const int r = r0 + hf * 8;
+      const float* brow = bias + (((size_t)(bw % nWb) * H + h) * N + (r < N ? r : 0)) * N;
+      float mx = -3.0e38f;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int col = 8 * j + c0 + e;
+          const float x = (col < N && r < N) ? fmaf(s[4 * j + 2 * hf + e], sl2, brow[col] * 1.4426950408889634f)
+                                             : -3.0e38f;
+          s[4 * j + 2 * hf + e] = x;
           mx = fmaxf(mx, x);
         }
-        float sum = 0.f;
+      }
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      float sum = 0.f;
 #pragma unroll
-        for (int j = 0; j < 64; ++j) {
-          const float e = (j < N) ? exp2f(v[j] - mx) : 0.f;
-          v[j] = e;
-          sum += e;
+      for (int j = 0; j < 8; ++j) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int col = 8 * j + c0 + e;
+          const float ex = (col < N && r < N) ? exp2f(s[4 * j + 2 * hf + e] - mx) : 0.f;
+          s[4 * j + 2 * hf + e] = ex;
+          sum += ex;
         }
-        inv = 1.f / sum;
+      }
+      sum += __shfl_xor_sync(0xffffffffu, sum, 1);
+      sum += __shfl_xor_sync(0xffffffffu, sum, 2);
+      inv[hf] = r < N ? 1.f / sum : 0.f;
 #pragma unroll
-        for (int c = 0; c < 8; ++c) {
-          uint4 pk;
-          __nv_bfloat162* hh = reinterpret_cast<__nv_bfloat162*>(&pk);
-#pragma unroll
-          for (int t = 0; t < 4; ++t) hh[t] = __floats2bfloat162_rn(v[c * 8 + 2 * t], v[c * 8 + 2 * t + 1]);
-          sts_128(sP + wa_swz(r, c), pk);
-        }
+      for (int j = 0; j < 8; ++j) {
+        const __nv_bfloat162 pk = __floats2bfloat162_rn(s[4 * j + 2 * hf], s[4 * j + 2 * hf + 1]);
+        // column 8j + c0 of row r: 16-byte chunk j, byte 2 * c0 inside it
+        *reinterpret_cast<__nv_bfloat162*>(smem + WA_SP + wa_swz(r, j) + c0 * 2) = pk;
       }
     }
     fence_proxy_async();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    if (tid == 0) {
+    float o[16];
 #pragma unroll
-      for (int k = 0; k < 4; ++k)                            // K = 64 keys -> four K = 16 steps
-        umma_f16(tmem + 64, make_smem_desc_sw128(sP + k * 32, 16, 1024), make_smem_desc_sw128(sVt + k * 32, 16, 1024),
-                 idesc_o, k != 0);
-      umma_commit(bar);
-    }
-    mbar_wait(bar, phase);
-    phase ^= 1;
-    tc_fence_after();
-    if (warp < 2) {
-      uint32_t o[32];
-      tmem_ld_32x32b_x32(tmem + 64 + (uint32_t(warp * 32) << 16), o);
-      tmem_ld_wait();
+    for (int j = 0; j < 16; ++j) o[j] = 0.f;
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k)                              // K = 64 keys -> four K = 16 steps
+      wgmma_m64n32k16<0, 0>(o, make_smem_desc_sw128(sP + k * 32, 16, 1024),
+                            make_smem_desc_sw128(sVt + k * 32, 16, 1024), 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+#pragma unroll
+    for (int j = 0; j < 16; ++j) reg_fence(o[j]);
+#pragma unroll
+    for (int hf = 0; hf < 2; ++hf) {
+      const int r = r0 + hf * 8;
       if (r < N) {
-        __nv_bfloat16* dst = out + ((size_t)bw * N + r) * H * D + (size_t)h * D;
+        __nv_bfloat16* dst = out + ((size_t)bw * N + r) * H * D + (size_t)h * D + c0;
 #pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          uint4 pk;
-          __nv_bfloat162* hh = reinterpret_cast<__nv_bfloat162*>(&pk);
-#pragma unroll
-          for (int t = 0; t < 4; ++t)
-            hh[t] = __floats2bfloat162_rn(__uint_as_float(o[c * 8 + 2 * t]) * inv,
-                                          __uint_as_float(o[c * 8 + 2 * t + 1]) * inv);
-          reinterpret_cast<uint4*>(dst)[c] = pk;
-        }
+        for (int j = 0; j < 4; ++j)
+          *reinterpret_cast<__nv_bfloat162*>(dst + 8 * j) =
+              __floats2bfloat162_rn(o[4 * j + 2 * hf] * inv[hf], o[4 * j + 2 * hf + 1] * inv[hf]);
       }
     }
-    tc_fence_before();
-    __syncthreads();                                         // operands / accumulators free for the next pair
-    tc_fence_after();
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem, 128);
+    __syncthreads();                                         // operands free for the next pair
   }
 }
 
@@ -1219,7 +1218,7 @@ __global__ void __launch_bounds__(64) window_attn_bwd_kernel(const T* qkv, const
   }
 }
 
-static inline int grid_for(size_t n_items, int threads, int cap = 148 * 8) {
+static inline int grid_for(size_t n_items, int threads, int cap = 132 * 8) {
   size_t b = (n_items + threads - 1) / threads;
   if (b < 1) b = 1;
   if (b > (size_t)cap) b = cap;
@@ -1232,15 +1231,17 @@ using namespace flpr;
 
 extern "C" {
 
+// stats_part (required with stats): 2 x 1056 floats of scratch (2 per block, at most 132 * 8 blocks).
 int flpr_fused_opt(int adam, float* p, const float* g, float* m, float* v, const float* Q, const float* R,
                    const float* G, void* p_bf16, float* stats, size_t n, float lr, float beta1, float beta2, float eps,
                    float wd, int step, float lam2, float lam1, float atten, float momentum, int penalty_ones,
-                   const float* hyper, float* anchor, float* anchor_m, float* anchor_v, cudaStream_t st) {
+                   const float* hyper, float* anchor, float* anchor_m, float* anchor_v, float* stats_part,
+                   cudaStream_t st) {
   bind_device_of(p);
   if (n % 4) return -2;
   OptArgs a;
   a.p = p; a.g = g; a.m = m; a.v = v; a.Q = Q; a.R = R; a.G = G;
-  a.p_bf16 = reinterpret_cast<__nv_bfloat16*>(p_bf16); a.stats = stats; a.n = n;
+  a.p_bf16 = reinterpret_cast<__nv_bfloat16*>(p_bf16); a.stats = stats; a.stats_part = stats_part; a.n = n;
   a.lr = lr; a.beta1 = beta1; a.beta2 = beta2; a.eps = eps; a.wd = wd;
   a.bc1 = 1.f - powf(beta1, (float)step);
   a.bc2_sqrt = sqrtf(1.f - powf(beta2, (float)step));
@@ -1250,9 +1251,11 @@ int flpr_fused_opt(int adam, float* p, const float* g, float* m, float* v, const
   if (a.anchor != nullptr && ((adam && (anchor_m == nullptr || anchor_v == nullptr)) ||
                               (!adam && momentum != 0.f && anchor_m == nullptr)))
     return -3;
+  if (stats != nullptr && stats_part == nullptr) return -4;
   const int grid = grid_for(n / 4, 256);
   if (adam) fused_opt_kernel<true><<<grid, 256, 0, st>>>(a);
   else fused_opt_kernel<false><<<grid, 256, 0, st>>>(a);
+  if (stats != nullptr) opt_stats_kernel<<<1, 32, 0, st>>>(stats_part, stats, grid, R != nullptr, G != nullptr);
   return (int)cudaGetLastError();
 }
 
@@ -1277,24 +1280,26 @@ int flpr_compose(const float* G, const float* A, float a, float* theta, void* th
   return (int)cudaGetLastError();
 }
 
-// in_bf16 / out_bf16 select the logits / dlogits dtypes. stats: float[2] (loss mean accum, correct count accum).
-int flpr_ce_label_smooth(const void* logits, const long long* target, void* dlogits, float* stats, int B, int C,
-                         long long ld, float eps, float grad_scale, int in_bf16, int out_bf16, cudaStream_t st) {
+// in_bf16 / out_bf16 select the logits / dlogits dtypes. stats: float[2] (loss mean accum, correct count accum);
+// row_part: float[2 B] scratch.
+int flpr_ce_label_smooth(const void* logits, const long long* target, void* dlogits, float* stats, float* row_part,
+                         int B, int C, long long ld, float eps, float grad_scale, int in_bf16, int out_bf16, cudaStream_t st) {
   if (in_bf16 && out_bf16)
     ce_ls_kernel<__nv_bfloat16, __nv_bfloat16><<<B, 256, 0, st>>>(
-        reinterpret_cast<const __nv_bfloat16*>(logits), target, reinterpret_cast<__nv_bfloat16*>(dlogits), stats, B, C,
+        reinterpret_cast<const __nv_bfloat16*>(logits), target, reinterpret_cast<__nv_bfloat16*>(dlogits), row_part, B, C,
         ld, eps, grad_scale);
   else if (in_bf16)
     ce_ls_kernel<__nv_bfloat16, float><<<B, 256, 0, st>>>(reinterpret_cast<const __nv_bfloat16*>(logits), target,
-                                                           reinterpret_cast<float*>(dlogits), stats, B, C, ld, eps,
+                                                           reinterpret_cast<float*>(dlogits), row_part, B, C, ld, eps,
                                                            grad_scale);
   else if (out_bf16)
     ce_ls_kernel<float, __nv_bfloat16><<<B, 256, 0, st>>>(reinterpret_cast<const float*>(logits), target,
-                                                           reinterpret_cast<__nv_bfloat16*>(dlogits), stats, B, C, ld,
+                                                           reinterpret_cast<__nv_bfloat16*>(dlogits), row_part, B, C, ld,
                                                            eps, grad_scale);
   else
     ce_ls_kernel<float, float><<<B, 256, 0, st>>>(reinterpret_cast<const float*>(logits), target,
-                                                   reinterpret_cast<float*>(dlogits), stats, B, C, ld, eps, grad_scale);
+                                                   reinterpret_cast<float*>(dlogits), row_part, B, C, ld, eps, grad_scale);
+  ce_stats_kernel<<<1, 32, 0, st>>>(row_part, stats, B);
   return (int)cudaGetLastError();
 }
 
@@ -1304,7 +1309,7 @@ static void bn_launch_geometry(int M, int C, dim3& grid, dim3& block, int& rpb) 
   int by = 1;                                         // row-lanes per block (power of two, <= 16)
   while (by * 2 * bx <= 256 && by < 16) by *= 2;
   const int gx = (c8n + bx - 1) / bx;
-  int gy = (148 * 4) / gx;
+  int gy = (132 * 4) / gx;
   if (gy < 1) gy = 1;
   rpb = (M + gy - 1) / gy;
   if (rpb < by * 4) rpb = by * 4;
@@ -1321,7 +1326,7 @@ int flpr_bn_partials_floats(int M, int C) {
 
 // `part` is scratch of flpr_bn_partials_floats(M, C) floats (no zeroing needed).
 // pre_part / pre_nparts: column partials [pre_nparts][2][C] already produced by the convolution's epilogue
-// (gemm_tcgen05.cu, `col_part`): the statistics pass over x is skipped.
+// (gemm_wgmma.cu, `col_part`): the statistics pass over x is skipped.
 int flpr_bn_fwd(const void* x, const float* gamma, const float* beta, const void* residual, void* y, float* part,
                 float* mean, float* rstd, float* scale, float* shift, float* running_mean,
                 float* running_var, int M, int C, float eps, float momentum, int relu, const float* pre_part,
@@ -1451,7 +1456,7 @@ int flpr_s2d_pad(const void* x, void* y, int B, int H, int W, cudaStream_t st) {
   bind_device_of(x);
   if ((H & 1) || (W & 1)) return -2;
   const size_t cells = (size_t)B * (H / 2 + 3) * (W / 2 + 3);
-  s2d_pad_kernel<<<grid_for(cells, 256, 148 * 16), 256, 0, st>>>(reinterpret_cast<const __nv_bfloat16*>(x),
+  s2d_pad_kernel<<<grid_for(cells, 256, 132 * 16), 256, 0, st>>>(reinterpret_cast<const __nv_bfloat16*>(x),
                                                                 reinterpret_cast<__nv_bfloat16*>(y), B, H, W);
   return (int)cudaGetLastError();
 }
@@ -1461,7 +1466,7 @@ int flpr_maxpool3x3s2(const void* x, void* y, int B, int H, int W, int C, cudaSt
   bind_device_of(x);
   if (C % 8) return -2;
   const size_t total = (size_t)B * ((H - 1) / 2 + 1) * ((W - 1) / 2 + 1) * (C / 8);
-  maxpool3x3s2_nhwc_kernel<<<grid_for(total, 256, 148 * 16), 256, 0, st>>>(
+  maxpool3x3s2_nhwc_kernel<<<grid_for(total, 256, 132 * 16), 256, 0, st>>>(
       reinterpret_cast<const __nv_bfloat16*>(x), reinterpret_cast<__nv_bfloat16*>(y), B, H, W, C);
   return (int)cudaGetLastError();
 }
@@ -1476,7 +1481,7 @@ int flpr_window_attn_fwd(const void* qkv, const float* bias, void* out, int BW, 
   if (N > ATT_MAXN || D > ATT_MAXD || N < 1) return -2;
   if (bf16 && D == 32 && g_window_attn_tc && (reinterpret_cast<uintptr_t>(qkv) & 15) == 0 &&
       (reinterpret_cast<uintptr_t>(out) & 15) == 0) {
-    // tensor-core path: persistent CTAs over (window, head) pairs, QK^T and PV on tcgen05 with TMEM accumulators
+    // tensor-core path: persistent CTAs over (window, head) pairs, QK^T and PV on wgmma
     static bool configured = false;
     if (!configured) {
       cudaError_t e = cudaFuncSetAttribute(window_attn_fwd_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -1485,7 +1490,7 @@ int flpr_window_attn_fwd(const void* qkv, const float* bias, void* out, int BW, 
       configured = true;
     }
     const long long pairs = (long long)BW * H;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const long long cap = (long long)sms * 4;

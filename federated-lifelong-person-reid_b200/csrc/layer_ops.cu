@@ -466,7 +466,7 @@ __global__ void __launch_bounds__(256) apply_global_kernel(const float4* __restr
 
 static int grid_for(long long work_items, int threads) {
   long long g = (work_items + threads - 1) / threads;
-  const long long cap = 148LL * 16;
+  const long long cap = 132LL * 16;
   if (g > cap) g = cap;
   if (g < 1) g = 1;
   return (int)g;
@@ -544,7 +544,7 @@ int flpr_ln_rows_train(const void* x, const float* gamma, const float* beta, voi
 // Blocks the backward kernel is launched with for `rows` rows (= rows of the partial buffer the caller allocates).
 int flpr_ln_rows_bwd_blocks(long long rows) {
   long long g = (rows + 7) / 8;
-  if (g > 148LL * 2) g = 148LL * 2;
+  if (g > 132LL * 2) g = 132LL * 2;
   if (g < 1) g = 1;
   return (int)g;
 }

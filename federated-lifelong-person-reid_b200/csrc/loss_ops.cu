@@ -1,12 +1,12 @@
 // flpr metric / distillation losses (criterions/triplet_loss.py:89-127, tools/distance.py:9-30,
-// criterions/kd_loss.py:10-27, methods/icarl.py:216-236 of the reference), fused around the tcgen05 Gram matrix:
+// criterions/kd_loss.py:10-27, methods/icarl.py:216-236 of the reference), fused around the wgmma Gram matrix:
 //
 //   triplet_mine_fwd   one block per anchor: distance row from the Gram matrix (squared euclidean  |xi|^2 + |xj|^2 -
 //                      2 G_ij  or cosine  1 - G_ij), positive / negative masks from the labels, hard (arg-max / arg-min)
 //                      or softmax-weighted mining -> dist_ap[i], dist_an[i] and the mining Jacobians
 //                      d dist_ap[i] / d dist[i,j],  d dist_an[i] / d dist[i,j]   (two B x B fp32 matrices).
 //   triplet_mine_bwd   W = g_ap (.) J_ap + g_an (.) J_an  ->  S = W + W^T (bf16, the operand of the gradient GEMM
-//                      dX = 2 (rowsum(S) (.) X - S X)  /  - S X  that runs on the tcgen05 kernel) and rowsum(S).
+//                      dX = 2 (rowsum(S) (.) X - S X)  /  - S X  that runs on the wgmma kernel) and rowsum(S).
 //   kd_kl              KL( softmax(t / T) || softmax(s / T) ) * T^2 / B  with gradient w.r.t. the student logits.
 //   bce_distill        iCaRL: BCEWithLogits(score, one-hot) + BCEWithLogits(score[:, :P], sigmoid(prev logits)),
 //                      mean-reduced, with gradient.
@@ -254,7 +254,7 @@ int flpr_bce_distill(const void* z, const long long* target, const float* prev, 
   bind_device_of(z);
   const long long n = (long long)B * C;
   int grid = (int)((n + 255) / 256);
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > 132 * 8) grid = 132 * 8;
   if (is_bf16)
     bce_distill_kernel<__nv_bfloat16><<<grid, 256, 0, st>>>(reinterpret_cast<const __nv_bfloat16*>(z), target, prev, dz,
                                                             loss, B, C, P, ldz, ldp);

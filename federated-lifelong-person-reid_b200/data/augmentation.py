@@ -51,7 +51,7 @@ class DeviceAugment:
         self.scale, self.ratio = scale, ratio
 
     def _native(self, u8: torch.Tensor, generator) -> torch.Tensor:
-        """One fused sm_100a kernel (``csrc/fused_ops.cu: augment_u8_kernel``): normalise + flip + erase + cast."""
+        """One fused sm_90a kernel (``csrc/fused_ops.cu: augment_u8_kernel``): normalise + flip + erase + cast."""
         import ctypes as C
         from ..ops import native
         lib = native.kernels()

@@ -7,8 +7,8 @@ conv+bias+residual+ReLU are single fused calls, and a whole trunk pass for a giv
 graph so that ~160 module dispatches per batch collapse into one launch.
 
 Execution paths of the residual stages (``native`` flag):
-* **native** (default on CUDA when the shapes fit): every 1x1 convolution is a tcgen05 GEMM and every 3x3 / strided
-  convolution an implicit GEMM of ``csrc/gemm_tcgen05.cu`` (NHWC bf16, folded-BN bias + residual + ReLU in the lean
+* **native** (default on CUDA when the shapes fit): every 1x1 convolution is a wgmma GEMM and every 3x3 / strided
+  convolution an implicit GEMM of ``csrc/gemm_wgmma.cu`` (NHWC bf16, folded-BN bias + residual + ReLU in the lean
   epilogue, stride 2 through TMA element strides) - the same kernels as the trainable head;
 * **library** fallback (cuDNN fused conv calls) for shapes the implicit-GEMM tiling does not cover.
 The 7x7 / 2 stem (3 input channels) runs natively as a 4x4 convolution over 2x2 space-to-depth cells
@@ -95,7 +95,7 @@ class FoldedTrunk:
             y = y + residual
         return F.relu_(y) if relu else y
 
-    # ------------------------------------------------------------------ native (tcgen05) residual stages
+    # ------------------------------------------------------------------ native (wgmma) residual stages
     def _prepare_native(self) -> None:
         """OHWI bf16 weights + fp32 biases for the implicit-GEMM kernels."""
         from ..ops.gemm import stem_weight_s2d
@@ -171,7 +171,7 @@ class FoldedTrunk:
         for op in self.ops:
             if op[0] == "conv_relu":
                 if native_stem:
-                    # 7x7 / 2 stem as a 4x4 conv over space-to-depth cells on the tcgen05 kernel (NHWC in, NHWC out)
+                    # 7x7 / 2 stem as a 4x4 conv over space-to-depth cells on the wgmma kernel (NHWC in, NHWC out)
                     x = gops.stem_conv(x.permute(0, 2, 3, 1).contiguous(), self._stem_w4, self._stem_bias, relu=True)
                 else:
                     x = self._conv(x, op[1], op[2], op[3], op[4], True)

@@ -4,10 +4,10 @@ Capability parity with ``models/resnet.py:45-344`` of the reference: the ``state
 naming (``base.conv1``, ``base.layer{1..4}.{i}.conv{j}|bn{j}|downsample.{0,1}``, ``bottleneck``, ``classifier``) so
 reference checkpoints load; train mode returns ``(cls_score, global_feat)``, eval mode returns ``global_feat``.
 
-B200-first differences:
+H100-first differences:
 * the network is explicitly split into a *frozen trunk* and a *trainable head* at the first fine-tuned stage
   (the reference discovers the same cut with two ``torch.fx`` traces, ``methods/fedstil.py:258-288``);
-* activations are NHWC bf16 on CUDA; the head runs on the tcgen05 GEMM / implicit-GEMM kernels
+* activations are NHWC bf16 on CUDA; the head runs on the wgmma GEMM / implicit-GEMM kernels
   (:mod:`flpr_b200.ops.gemm`) with fused batch-norm kernels, the trunk runs inference-only with folded BN;
 * no network access: ImageNet weights are loaded from ``pretrained_path`` when given, else random init.
 """
@@ -168,7 +168,7 @@ class ResNetReID(nn.Module):
 
     def forward_trunk(self, x: torch.Tensor) -> torch.Tensor:
         """Frozen part: input image batch -> feature map at the cut ("prototype" in FedSTIL terms).
-        On CUDA with a bf16 fast head the frozen stages run on the tcgen05 kernels too (:class:`NativeTrunk`) - in
+        On CUDA with a bf16 fast head the frozen stages run on the wgmma kernels too (:class:`NativeTrunk`) - in
         train mode with batch-statistic BN and running-stat updates, which is what the reference's ``model.train()``
         does to the whole net for every method but FedSTIL (``methods/baseline.py:38``, ``models/resnet.py:229-241``)."""
         nt = getattr(self, "_native_trunk", None)
@@ -211,7 +211,7 @@ class ResNetReID(nn.Module):
 
 # ------------------------------------------------------------------------------------------------- fast head
 class FastResNetHead:
-    """tcgen05 execution of ``layer{k..4}`` + GAP + BNNeck + classifier over NHWC bf16 activations.
+    """wgmma execution of ``layer{k..4}`` + GAP + BNNeck + classifier over NHWC bf16 activations.
 
     Shares the ``nn.Parameter`` objects of the wrapped model (weights must be in ``channels_last`` memory format so
     that the OHWI view is contiguous) and an optional bf16 shadow provider ``shadow(param) -> bf16 tensor`` kept in
@@ -394,7 +394,7 @@ class FastResNetHead:
 
 
 class NativeTrunk(FastResNetHead):
-    """The frozen stages (stem + ``layer1..k-1``) on the tcgen05 kernels, forward only - nothing in them is trainable
+    """The frozen stages (stem + ``layer1..k-1``) on the wgmma kernels, forward only - nothing in them is trainable
     and their input does not require grad, so no autograd graph is built. ``model.train()``: every BatchNorm
     normalises with the batch statistics that the producing convolution's epilogue emitted and updates its running
     statistics (``bn_finalize``); ``model.eval()``: running statistics (``affine_act``).

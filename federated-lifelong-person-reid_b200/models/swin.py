@@ -5,7 +5,7 @@ bias, patch merging, stochastic depth, optional activation checkpointing, 224x22
 Parameter names follow timm's (``base.patch_embed.proj``, ``base.layers.{i}.blocks.{j}.attn.qkv`` ...), so
 ``fine_tuning: [base.layers.3, classifier]`` and reference checkpoints address the same tensors.
 
-Written from the architecture description, not from the reference source. B200-first choices: the attention core is
+Written from the architecture description, not from the reference source. H100-first choices: the attention core is
 one fused ``scaled_dot_product_attention`` call per block with the relative-position bias and the shift mask merged
 into a single additive bias tensor that is cached per (window grid, shift); window (un)partition is a pure reshape /
 permute pair; the network exposes the same *frozen trunk | trainable head* split as the ResNets
@@ -34,7 +34,7 @@ from ..ops import layer as lops  # noqa: E402
 
 
 class TcLinear(nn.Linear):
-    """``nn.Linear`` whose CUDA / bf16 forward, data gradient and weight gradient run on the tcgen05 GEMM kernel
+    """``nn.Linear`` whose CUDA / bf16 forward, data gradient and weight gradient run on the wgmma GEMM kernel
     (``ops.gemm.linear``: bf16 compute copy of the weight kept by the fused optimizer, fp32 weight gradient written by
     the GEMM epilogue straight into the parameter's slot of the arena gradient buffer). Same parameters, same
     ``state_dict`` keys: an existing ``nn.Linear`` is switched over by re-classing it (:func:`use_tensor_core_linears`).
@@ -83,8 +83,8 @@ class FrozenLayerNorm(nn.LayerNorm):
         c = x.shape[-1]
         if c % 8 == 0 and c <= 2048 and len(self.normalized_shape) == 1 and w.dtype == torch.float32 \
                 and self.bias is not None and lops.enabled("swin_tokens", x.device):
-            # native warp-per-token kernel (fp32 statistics, fp32 gamma / beta): ATen's bf16 LayerNorm was 1.9 ms of the
-            # 6.3 ms Swin-T trunk forward (profiles/r2_results.md) for ~0.15 ms worth of HBM traffic
+            # native warp-per-token kernel (fp32 statistics, fp32 gamma / beta): one pass over the tokens where ATen's
+            # bf16 LayerNorm takes several
             x2 = x.reshape(-1, c)
             return lops.ln_rows(x2 if x2.is_contiguous() else x2.contiguous(), self.weight, self.bias,
                                 self.eps).view(x.shape)

@@ -19,6 +19,12 @@ _stream = native.stream_of
 
 
 # --------------------------------------------------------------------------------------------- optimizers
+def _opt_stats_scratch(device) -> torch.Tensor:
+    """Per-block partials of the optimizer's penalty statistics (2 per block, at most 132 * 8 blocks), summed by the
+    library in block order so that the reported penalty is reproducible."""
+    return torch.empty(2 * 132 * 8, dtype=torch.float32, device=device)
+
+
 def fused_optimizer_step(kind: str, p: torch.Tensor, g: torch.Tensor, m: Optional[torch.Tensor],
                          v: Optional[torch.Tensor], *, lr: float, step: int, beta1: float = 0.9, beta2: float = 0.999,
                          eps: float = 1e-8, weight_decay: float = 0.0, momentum: float = 0.0,
@@ -78,7 +84,8 @@ def fused_optimizer_step(kind: str, p: torch.Tensor, g: torch.Tensor, m: Optiona
                             native.ptr(R), native.ptr(G), native.ptr(p_bf16), native.ptr(stats), p.numel(), lr, beta1,
                             beta2, eps, weight_decay, int(step), lam2, lam1, atten, momentum, int(penalty_ones),
                             native.ptr(hyper), native.ptr(anchor if G is not None else None), native.ptr(anchor_m),
-                            native.ptr(anchor_v), _stream(p.device))
+                            native.ptr(anchor_v), native.ptr(None if stats is None else _opt_stats_scratch(p.device)),
+                            _stream(p.device))
     native.check(rc, "flpr_fused_opt")
     native.count_launch()
 
@@ -139,15 +146,16 @@ class _CELabelSmoothFn(torch.autograd.Function):
     def forward(ctx, logits, target, eps, stats):
         b, c = logits.shape
         dlogits = torch.empty_like(logits)
-        local = torch.zeros(2, dtype=torch.float32, device=logits.device)
+        local = torch.zeros(2 + 2 * b, dtype=torch.float32, device=logits.device)   # [loss, hits] + per-row scratch
         lib = _lib()
-        rc = lib.flpr_ce_label_smooth(native.ptr(logits), native.ptr(target), native.ptr(dlogits), native.ptr(local), b,
+        rc = lib.flpr_ce_label_smooth(native.ptr(logits), native.ptr(target), native.ptr(dlogits), native.ptr(local),
+                                      native.ptr(local[2:]), b,
                                       c, logits.stride(0), eps, 1.0 / b, int(logits.dtype == torch.bfloat16),
                                       int(dlogits.dtype == torch.bfloat16), _stream(logits.device))
         native.check(rc, "flpr_ce_label_smooth")
         native.count_launch()
         if stats is not None:
-            stats += local
+            stats += local[:2]
         ctx.save_for_backward(dlogits)
         return local[0]
 
@@ -378,9 +386,9 @@ def window_attention(qkv: torch.Tensor, bias: torch.Tensor, scale: float) -> tor
 # --------------------------------------------------------------------------------------------- metric / KD losses
 class _MinedDistancesFn(torch.autograd.Function):
     """``(dist_ap, dist_an)`` of the fast-reid triplet loss (``criterions/triplet_loss.py:89-127``): Gram matrix on the
-    tcgen05 GEMM (bf16 hi / lo split: ~fp32 accuracy, the distances are differences of large numbers), distance row +
+    wgmma GEMM (bf16 hi / lo split: ~fp32 accuracy, the distances are differences of large numbers), distance row +
     masks + hard / softmax-weighted mining in one kernel per anchor; backward = one small kernel that folds the mining
-    Jacobians with the incoming gradients into ``S = W + W^T`` and ONE tcgen05 GEMM ``S @ X``."""
+    Jacobians with the incoming gradients into ``S = W + W^T`` and ONE wgmma GEMM ``S @ X``."""
 
     @staticmethod
     def forward(ctx, x, labels, cosine, hard):

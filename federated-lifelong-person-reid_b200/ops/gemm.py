@@ -1,4 +1,4 @@
-"""Tensor-core GEMM / implicit-GEMM convolution ops (``csrc/gemm_tcgen05.cu``) and their autograd wrappers.
+"""Tensor-core GEMM / implicit-GEMM convolution ops (``csrc/gemm_wgmma.cu``) and their autograd wrappers.
 
 Layout conventions: activations are NHWC bf16 flattened to ``[pixels, channels]``; weights are ``[out, in]`` (1x1 /
 linear) or ``[out, kh, kw, in]`` (3x3, "OHWI"), i.e. the reduction dim is always contiguous in the forward pass. The
@@ -30,6 +30,13 @@ def col_part_buffer(m: int, n: int, device) -> torch.Tensor:
     return torch.empty(col_part_rows(m), 2, n, dtype=torch.float32, device=device)
 
 
+def _split_workspace(split: int, rows: int, ld: int, device) -> Optional[torch.Tensor]:
+    """Partial-product slices of a split-K GEMM (reduced in split order by the library: bitwise reproducible)."""
+    if split <= 1:
+        return None
+    return torch.empty(split * ((rows * ld + 3) // 4 * 4), dtype=torch.float32, device=device)
+
+
 def _col_part_reference(d: torch.Tensor, col_part: torch.Tensor) -> None:
     """CPU reference of the fused statistics: 32-row partial sums of ``d`` and ``d*d``."""
     m, n = d.shape
@@ -49,7 +56,8 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_kmajor: bool = True, b_kmajor: b
     """``D[M,N] = alpha * A @ B^T`` with bf16 operands and fp32 accumulation.
 
     ``a`` is ``[M,K]`` (``a_kmajor``) or ``[K,M]``; ``b`` is ``[N,K]`` (``b_kmajor``) or ``[K,N]``.
-    Returns ``[M,N]`` (``[N,M]`` when ``trans_out``). ``split_k > 1`` accumulates atomically into a zeroed fp32 output.
+    Returns ``[M,N]`` (``[N,M]`` when ``trans_out``). ``split_k > 1`` accumulates into a zeroed fp32 output (the
+    splits are summed in a fixed order, so the result is reproducible).
     ``col_part`` (fp32 ``[ceil(M/128)*4, 2, N]``, see :func:`col_part_buffer`) receives per-32-row partial column
     sums / sums of squares of the fp32 result: the batch-norm statistics pass over the output is fused away.
     """
@@ -98,6 +106,7 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_kmajor: bool = True, b_kmajor: b
                             0 if a_kmajor else 1, 0 if b_kmajor else 1, int(out.dtype == torch.bfloat16),
                             int(trans_out), float(alpha), native.ptr(bias_n), native.ptr(bias_m), int(relu),
                             native.ptr(residual), int(split_k), int(bn), native.ptr(col_part),
+                            native.ptr(_split_workspace(split_k, oshape[0], out.stride(0), a.device)),
                             native.stream(a.device))
     native.check(rc, "flpr_gemm_bf16")
     native.count_launch()
@@ -185,7 +194,7 @@ def _auto_split(m: int, n: int, k: int, taps: int = 1) -> int:
     kb = (k + 63) // 64
     if tiles >= 120 or kb < 8:
         return 1
-    return max(1, min(kb // 4, (148 + tiles - 1) // tiles))
+    return max(1, min(kb // 4, (132 + tiles - 1) // tiles))
 
 
 class _LinearFn(torch.autograd.Function):
@@ -251,7 +260,7 @@ def linear(x: torch.Tensor, w_master: torch.Tensor, w_bf16: Optional[torch.Tenso
 
 
 class _Conv3x3Fn(torch.autograd.Function):
-    """3x3 / stride 1 / pad 1 NHWC convolution: forward, dgrad and wgrad all on the tcgen05 implicit-GEMM kernel."""
+    """3x3 / stride 1 / pad 1 NHWC convolution: forward, dgrad and wgrad all on the wgmma implicit-GEMM kernel."""
 
     @staticmethod
     def forward(ctx, x, w_master, w_bf16, grad_out, want_stats=False):
@@ -306,7 +315,8 @@ def conv3x3_wgrad(x: torch.Tensor, dy: torch.Tensor, out: Optional[torch.Tensor]
         out = torch.zeros((cout, 3, 3, cin), dtype=torch.float32, device=x.device)
     assert out.is_contiguous() and out.dtype == torch.float32 and out.numel() == cout * 9 * cin
     rc = lib.flpr_conv_wgrad_nhwc_bf16(native.ptr(x), native.ptr(dy), native.ptr(out), n, h, w, cin, cout, 3, 3, 1, 1,
-                                       int(split), 0, native.stream(x.device))
+                                       int(split), 0, native.ptr(_split_workspace(split, cout, 9 * cin, x.device)),
+                                       native.stream(x.device))
     native.check(rc, "flpr_conv_wgrad_nhwc_bf16")
     native.count_launch()
     return out
@@ -334,7 +344,7 @@ def zero_stuff2(t: torch.Tensor, h: int, w: int) -> torch.Tensor:
 
 def conv_s2_supported(h: int, w: int, cin: int, cout: int, k: int) -> bool:
     """Shapes for which forward, data gradient and weight gradient of a ``k x k`` / stride-2 / pad ``k//2``
-    convolution all run on the tcgen05 kernels (:class:`_ConvStride2Fn`)."""
+    convolution all run on the wgmma kernels (:class:`_ConvStride2Fn`)."""
     if k == 1:
         return cin % 8 == 0 and cout % 8 == 0 and conv_supported(h, w, cin, 1, 2, 0)
     if k != 3:
@@ -346,7 +356,7 @@ def conv_s2_supported(h: int, w: int, cin: int, cout: int, k: int) -> bool:
 
 
 class _ConvStride2Fn(torch.autograd.Function):
-    """``k x k`` (k = 1 or 3) / stride 2 / pad ``k//2`` NHWC convolution with every pass on the tcgen05 kernels.
+    """``k x k`` (k = 1 or 3) / stride 2 / pad ``k//2`` NHWC convolution with every pass on the wgmma kernels.
 
     Forward: the implicit-GEMM kernel walks the input with TMA element strides. Backward: a stride-2 convolution is
     its stride-1 parent sampled at the even output positions (``y[i] = z[2i]``), so ``dL/dz`` is ``dy`` zero-stuffed

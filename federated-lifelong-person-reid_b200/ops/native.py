@@ -1,4 +1,4 @@
-"""ctypes bindings for ``lib/libflpr_b200.so`` (the sm_100a kernels in ``csrc/``).
+"""ctypes bindings for ``lib/libflpr_b200.so`` (the sm_90a kernels in ``csrc/``).
 
 Policy: on a CUDA tensor every op in :mod:`flpr_b200.ops` goes through the native library and raises loudly if the
 library is missing or a launch fails — there is no silent eager fallback on a GPU box. On CPU tensors the ops use a
@@ -36,10 +36,10 @@ def available() -> bool:
 def _signatures() -> dict:
     P, I, F, Z, L, D = c_void_p, c_int, c_float, c_size_t, c_ll, c_double
     return {
-        "flpr_gemm_bf16": [P, P, P, I, I, I, L, L, L, I, I, I, I, F, P, P, I, P, I, I, P, P],
+        "flpr_gemm_bf16": [P, P, P, I, I, I, L, L, L, I, I, I, I, F, P, P, I, P, I, I, P, P, P],
         "flpr_conv_nhwc_bf16": [P, P, P, I, I, I, I, I, I, I, I, I, I, F, P, I, P, I, P, I, L, L, L, P],
         "flpr_conv_dgrad_nhwc_bf16": [P, P, P, I, I, I, I, I, I, I, I, I, I, I, P],
-        "flpr_conv_wgrad_nhwc_bf16": [P, P, P, I, I, I, I, I, I, I, I, I, I, I, P],
+        "flpr_conv_wgrad_nhwc_bf16": [P, P, P, I, I, I, I, I, I, I, I, I, I, I, P, P],
         "flpr_symm_alloc": [C.POINTER(P), Z],
         "flpr_symm_free": [P],
         "flpr_ipc_get_handle": [P, P],
@@ -56,11 +56,11 @@ def _signatures() -> dict:
         "flpr_comm_curv_moments": [I, I, P, D, I, P, P, P, P, P, Z, I, P],
         "flpr_comm_gather_strided": [I, I, P, D, I, P, P, Z, I, P],
         "flpr_comm_pull_copy": [I, I, P, D, P, P, P, Z, I, P],
-        "flpr_fused_opt": [I, P, P, P, P, P, P, P, P, P, Z, F, F, F, F, F, I, F, F, F, F, I, P, P, P, P, P],
+        "flpr_fused_opt": [I, P, P, P, P, P, P, P, P, P, Z, F, F, F, F, F, I, F, F, F, F, I, P, P, P, P, P, P],
         "flpr_importance_accum": [P, P, Z, F, I, P],
         "flpr_cast_bf16": [P, P, Z, P],
         "flpr_compose": [P, P, F, P, P, Z, P],
-        "flpr_ce_label_smooth": [P, P, P, P, I, I, L, F, F, I, I, P],
+        "flpr_ce_label_smooth": [P, P, P, P, P, I, I, L, F, F, I, I, P],
         "flpr_bn_fwd": [P, P, P, P, P, P, P, P, P, P, P, P, I, I, F, F, I, P, I, P],
         "flpr_affine_act": [P, P, P, P, P, I, I, I, P],
         "flpr_bn_bwd": [P, P, P, P, P, P, P, P, P, P, P, I, I, I, I, P],

@@ -79,7 +79,7 @@ class FedComm:
         self.backend = mode
         if self.mode == "p2p":
             self._init_p2p()
-            self.comm_blocks = comm_blocks or 148 * 2
+            self.comm_blocks = comm_blocks or 132 * 2
         else:
             self._arena = torch.zeros(self.arena_bytes, dtype=torch.uint8, device=self.device)
             self.comm_blocks = 0

@@ -4,7 +4,7 @@ Every client keeps its trainable state in ONE contiguous fp32 buffer (``master``
 autograd accumulates into in place, an optional bf16 compute copy (``shadow``) refreshed by the optimizer kernel, and
 the optimizer moments. Named ``nn.Parameter`` objects are *views* into the arena, so the reference's dict schemas are
 reconstructed only at checkpoint / payload time (SURVEY §7.1). On CUDA, conv weights are laid out OHWI
-(``channels_last``) so the tcgen05 implicit-GEMM kernels read them without any per-step transpose; a CPU arena keeps
+(``channels_last``) so the wgmma implicit-GEMM kernels read them without any per-step transpose; a CPU arena keeps
 the standard OIHW order, which makes the fp32 CPU path run the very same ATen kernels as the reference (the
 whole-experiment golden tests rely on that).
 

@@ -1,9 +1,9 @@
 """Checkpoint files as persistent, CUDA-registered file mappings: a snapshot is a set of DMAs straight into the file.
 
 The asynchronous :class:`~.checkpoint.CheckpointStore` moves a snapshot device -> pinned arena -> writer process ->
-``torch.save`` -> fresh RAM-disk pages. At 8 GPUs the federated round produces 6.5 GB of reference-layout files per
-90 ms, and the *host* side of that pipeline (page allocation + one CPU copy per byte, ~30 GB/s box-wide) becomes what
-bounds the round (``profiles/r2_scaling.md``). Here the host CPU does not touch the payload at all:
+``torch.save`` -> fresh RAM-disk pages. The federated round produces several GB of reference-layout files, and at
+8 GPUs the *host* side of that pipeline (page allocation + one CPU copy per byte) can bound the round. Here the host
+CPU does not touch the payload at all:
 
 * The byte layout of a checkpoint file is a pure function of the state's *structure* (keys, shapes, dtypes): the
   legacy ``torch.save`` container is ``[pickles: magic, protocol, sys-info, object graph, storage keys]`` followed by

@@ -94,7 +94,7 @@ class ModelModule(nn.Module):
             from ..models.swin import SwinTransformerReID, use_tensor_core_linears
             if isinstance(self.net, SwinTransformerReID) and getattr(self, "use_tc_linears", True):
                 # every Linear of the backbone (qkv / proj / fc1 / fc2 / patch merging) and the classifier on the
-                # tcgen05 GEMM: trainable ones with the optimizer-maintained bf16 copy and direct gradient slots
+                # wgmma GEMM: trainable ones with the optimizer-maintained bf16 copy and direct gradient slots
                 use_tensor_core_linears(self.net, self.arena.shadow_of, self.arena.grad_of)
                 from ..ops import layer as lops
                 lops.enabled("swin_tokens", device)    # one-time on-device self-check of the token kernels, up front

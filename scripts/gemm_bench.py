@@ -1,4 +1,4 @@
-"""Isolated timing of the tcgen05 GEMM on the head-step shapes: persistent vs classic kernel, tile widths, fused
+"""Isolated timing of the wgmma GEMM on the head-step shapes: persistent vs classic kernel, tile widths, fused
 statistics on/off, next to torch.matmul (cuBLAS) on the same shapes. CUDA events, L2 flushed between iterations."""
 import os, sys, math
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

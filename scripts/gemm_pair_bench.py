@@ -1,4 +1,4 @@
-"""CTA-pair (cta_group::2) kernel vs the single-CTA persistent kernel on the head-step shapes."""
+"""CTA-pair kernel (2-CTA clusters, B tile multicast) vs the single-CTA persistent kernel on the head-step shapes."""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)

@@ -3,8 +3,8 @@
     ncu --set full --clock-control none --import-source on -k regex:<pattern> -c 4 -o gpurun_out/prof_<x> \
         python scripts/ncu_targets.py <what>
 
-what: head (FedSTIL ResNet-50 head step: tcgen05 GEMM / conv fwd, dgrad, wgrad, BN, CE, fused Adam + trained anchor),
-      trunk (native train-mode trunk: stem, strided convs, batch-stat BN), swin (tcgen05 window attention + TcLinear),
+what: head (FedSTIL ResNet-50 head step: wgmma GEMM / conv fwd, dgrad, wgrad, BN, CE, fused Adam + trained anchor),
+      trunk (native train-mode trunk: stem, strided convs, batch-stat BN), swin (wgmma window attention + TcLinear),
       comm (fed_mix / fed_reduce_bcast / gather on one GPU), misc (triplet mining, herding, augmentation, rank_eval).
 """
 import os, sys

@@ -1,4 +1,4 @@
-"""Static resource table of every kernel (``nvcc -Xptxas -v``, cross-compiled for sm_100a; no GPU needed):
+"""Static resource table of every kernel (``nvcc -Xptxas -v``, cross-compiled for sm_90a; no GPU needed):
 registers, static shared memory, spills, and the occupancy the register / launch-bound pair allows.
 
     python scripts/ptxas_resources.py        # -> profiles/ptxas_resources.md
@@ -25,7 +25,7 @@ def main():
         assert r.returncode == 0, r.stderr[-2000:]
         cur = None
         for line in r.stderr.splitlines():
-            m = re.search(r"Compiling entry function '([^']+)' for 'sm_100a'", line)
+            m = re.search(r"Compiling entry function '([^']+)' for 'sm_90a'", line)
             if m:
                 cur = {"src": src, "name": m.group(1), "spill_st": 0, "spill_ld": 0, "stack": 0}
                 rows.append(cur)
@@ -42,9 +42,9 @@ def main():
                 sm = re.search(r"(\d+) bytes smem", line)
                 cur["smem"] = int(sm.group(1)) if sm else 0
     names = demangle([r["name"] for r in rows])
-    out = ["# Kernel resources (`nvcc -Xptxas -v`, sm_100a)", "",
+    out = ["# Kernel resources (`nvcc -Xptxas -v`, sm_90a)", "",
            "Static view of every `__global__` entry of `csrc/*.cu` (dynamic shared memory - the TMA stage rings of the",
-           "tcgen05 kernels - is requested at launch and not part of this table). `spill` is stores/loads in bytes;",
+           "wgmma kernels - is requested at launch and not part of this table). `spill` is stores/loads in bytes;",
            "the notes under the table say which instantiations run on the hot path.", "",
            "| source | kernel | regs | static smem (B) | barriers | stack (B) | spill st/ld (B) |", "|---|---|---|---|---|---|---|"]
     spills = 0
@@ -55,16 +55,9 @@ def main():
         spills += (r["spill_st"] + r["spill_ld"]) > 0
     out += ["", f"{len(rows)} entry points, {spills} with register spills.", "",
             "Notes", "",
-            "* `gemm_bf16_tcgen05_pair_kernel` (CTA pair, `cta_group::2`, the conv / large-GEMM path of the head step and",
-            "  the native trunk) and every kernel of `fedcomm.cu`, `fused_ops.cu`, `loss_ops.cu`: no spills.",
-            "* `gemm_bf16_tcgen05_persistent_kernel<BN=64|128,...>`: 12 B / 20 B of spill traffic in the epilogue warps under",
-            "  `__launch_bounds__(.., 2)` (two CTAs per SM so that one tile's epilogue hides under the other's main loop;",
-            "  128-register cap). The spilled values are loop-invariant addresses reloaded once per tile.",
-            "* `<BN=256,...>` (one CTA per SM, 168 registers): 96 B / 160 B; the `<256, 1, 2>` instantiation (MN-major A x",
-            "  implicit-GEMM B = wgrad) spills 456 B / 708 B; wgrad of the ResNet / Swin layers takes the spill-free pair",
-            "  kernel (`pair_ok`), this instantiation is the fallback for shapes the pair kernel refuses.",
             "* template arguments: `<BN, A operand mode, B operand mode, epilogue>`; operand modes 0 = K-major, 1 = MN-major,",
             "  2 = implicit-GEMM convolution (TMA im2col walk), 3 = tap-flipped convolution (dgrad)."]
+    os.makedirs(os.path.join(ROOT, "profiles"), exist_ok=True)
     path = os.path.join(ROOT, "profiles", "ptxas_resources.md")
     with open(path, "w") as f:
         f.write("\n".join(out) + "\n")

@@ -4,14 +4,14 @@
 # The selection keeps the instrumented run short; the full suite is `pytest tests/test_gpu_kernels.py`.
 #
 # racecheck / synccheck target the kernels whose correctness rests on shared-memory hand-offs and barriers:
-#   * tcgen05 GEMM family: TMA -> mbarrier -> MMA -> tcgen05.commit -> epilogue staging tile (smem reuse across tiles)
+#   * wgmma GEMM family: TMA -> mbarrier -> wgmma -> accumulator + epilogue staging tiles (smem reuse across tiles)
 #   * window_attn_fwd_tc: Q/K/V^T staging, P written back to smem between the two MMAs
 #   * BN / CE / herding / triplet kernels: block reductions through shared memory
 #   * fedcomm single-rank: the intra-block part of rank_barrier (__syncthreads_or around the flag spin)
 # (the cross-rank flag protocol itself is system-scope global memory: racecheck does not model it; it is covered by
 #  tests/dist_comm_check.py and scripts/comm_soak.py)
 TOOL=${1:-memcheck}
-SEL=${2:-"test_gemm_kmajor and 256-512-512 or test_conv_nhwc and 3-4-16-8 or test_lean_epilogue and 4096 or test_strided and 4-64-32-128 or test_fused_optimizer or test_fused_trained_l1_anchor or test_herding or test_fused_augmentation and default-dtype0 or test_comm_single_rank or test_window_attention_tcgen05_forward and 37 or test_fused_triplet_loss and True-True or test_fused_kd_and_bce or test_batch_norm_shapes"}
+SEL=${2:-"test_gemm_kmajor and 256-512-512 or test_conv_nhwc and 3-4-16-8 or test_lean_epilogue and 4096 or test_strided and 4-64-32-128 or test_fused_optimizer or test_fused_trained_l1_anchor or test_herding or test_fused_augmentation and default-dtype0 or test_comm_single_rank or test_window_attention_wgmma_forward and 37 or test_fused_triplet_loss and True-True or test_fused_kd_and_bce or test_batch_norm_shapes"}
 mkdir -p gpurun_out
 run() {
   local tool=$1

@@ -28,7 +28,7 @@ for tc in (0, 1):
     for _ in range(5):
         trunk()
     torch.cuda.synchronize()
-    print(f"trunk fwd, batch 64, tcgen05 attention {'on' if tc else 'off'}: {(time.perf_counter() - t0) / 5 * 1e3:.2f} ms wall")
+    print(f"trunk fwd, batch 64, wgmma attention {'on' if tc else 'off'}: {(time.perf_counter() - t0) / 5 * 1e3:.2f} ms wall")
 with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
     trunk()
     torch.cuda.synchronize()

@@ -8,24 +8,9 @@ if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
 
-def _ensure_reference_installed() -> None:
-    """``baseline/_ref`` (the unmodified reference the parity / golden tests use as their oracle) is git-ignored: a fresh
-    checkout re-creates it from ``/root/reference`` when that tree exists (``scripts/install_reference.sh``)."""
-    import subprocess
-    if os.path.isdir(os.path.join(ROOT, "baseline", "_ref", "methods")) or not os.path.isdir("/root/reference/methods"):
-        return
-    if os.environ.get("PYTEST_XDIST_WORKER"):          # the controller process installs; workers start afterwards
-        return
-    try:
-        subprocess.run(["bash", os.path.join(ROOT, "scripts", "install_reference.sh")], check=True, timeout=600,
-                       stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL)
-    except Exception as ex:  # noqa: BLE001  (the parity tests then skip, as before)
-        print(f"[conftest] reference install failed: {ex}")
-
-
 def _ensure_native_library() -> None:
     """``lib/libflpr_b200.so`` is git-ignored: a fresh checkout builds it before the first test needs it (``nvcc``
-    cross-compiles for sm_100a without a GPU; about a minute). A current library is left alone."""
+    cross-compiles for sm_90a without a GPU; about a minute). A current library is left alone."""
     if os.environ.get("PYTEST_XDIST_WORKER"):
         return
     try:
@@ -37,9 +22,8 @@ def _ensure_native_library() -> None:
 
 
 def pytest_configure(config):
-    _ensure_reference_installed()
     _ensure_native_library()
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device")
     config.addinivalue_line("markers", "multigpu: test needs >= 2 CUDA devices")
 
 

@@ -511,27 +511,20 @@ static inline float warp_max(float v) {
   for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
 }
-// tcgen05 / TMEM / mbarrier helpers of ptx.cuh: declared so that a source which ALSO contains a tensor-core kernel compiles
+// wgmma / shared-space helpers of ptx.cuh: declared so that a source which ALSO contains a tensor-core kernel compiles
 static inline uint32_t smem_u32(const void*) { flpr_emu::unsupported("cvta.shared"); }
-static inline void fence_mbar_init() { flpr_emu::unsupported("fence.mbarrier_init"); }
 static inline void fence_proxy_async() { flpr_emu::unsupported("fence.proxy.async"); }
 static inline uint64_t make_smem_desc_sw128(uint32_t, uint32_t, uint32_t) { flpr_emu::unsupported("smem descriptor"); }
-static inline void mbar_init(uint64_t*, uint32_t) { flpr_emu::unsupported("mbarrier.init"); }
-static inline void mbar_wait(uint64_t*, uint32_t) { flpr_emu::unsupported("mbarrier.try_wait"); }
 static inline void sts_128(uint32_t, const uint4&) { flpr_emu::unsupported("st.shared.v4"); }
-static inline void tc_fence_after() { flpr_emu::unsupported("tcgen05.fence"); }
-static inline void tc_fence_before() { flpr_emu::unsupported("tcgen05.fence"); }
-static inline void tmem_alloc(uint32_t*, uint32_t) { flpr_emu::unsupported("tcgen05.alloc"); }
-static inline void tmem_dealloc(uint32_t, uint32_t) { flpr_emu::unsupported("tcgen05.dealloc"); }
-static inline void tmem_ld_32x32b_x32(uint32_t, uint32_t (&)[32]) { flpr_emu::unsupported("tcgen05.ld"); }
-static inline void tmem_ld_wait() { flpr_emu::unsupported("tcgen05.wait"); }
-static inline void tmem_relinquish() { flpr_emu::unsupported("tcgen05.relinquish_alloc_permit"); }
-static inline void umma_commit(uint64_t*) { flpr_emu::unsupported("tcgen05.commit"); }
-static inline void umma_f16(uint32_t, uint64_t, uint64_t, uint32_t, uint32_t) { flpr_emu::unsupported("tcgen05.mma"); }
-constexpr uint32_t make_idesc_bf16(int m, int n, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) |
-         ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
-}
+static inline void reg_fence(float&) { flpr_emu::unsupported("wgmma register fence"); }
+static inline void wgmma_fence() { flpr_emu::unsupported("wgmma.fence"); }
+static inline void wgmma_commit() { flpr_emu::unsupported("wgmma.commit_group"); }
+template <int N>
+static inline void wgmma_wait() { flpr_emu::unsupported("wgmma.wait_group"); }
+template <int TA, int TB>
+static inline void wgmma_m64n64k16(float (&)[32], uint64_t, uint64_t, uint32_t) { flpr_emu::unsupported("wgmma"); }
+template <int TA, int TB>
+static inline void wgmma_m64n32k16(float (&)[16], uint64_t, uint64_t, uint32_t) { flpr_emu::unsupported("wgmma"); }
 // system-scope flag accesses: the spin loops of the peer-memory protocol are cooperative here
 static inline void st_release_sys(uint32_t* p, uint32_t v) {
   flpr_emu::maybe_yield();

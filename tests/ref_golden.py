@@ -1,4 +1,4 @@
-"""Runs a whole (tiny) experiment of the UNMODIFIED reference in baseline/_ref as a golden oracle.
+"""Runs a whole (tiny) experiment of the UNMODIFIED reference in oracle/_ref as a golden oracle.
 
     python tests/ref_golden.py <in.pt> <out.pt>
 
@@ -14,7 +14,7 @@ import sys
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.path.join(ROOT, "baseline", "_ref")
+REF = os.path.join(ROOT, "oracle", "_ref")
 sys.path.insert(0, ROOT)
 from baseline.reference_arm import _MemoryPipeline  # noqa: E402  (duck-typed pipeline, no reference import inside)
 

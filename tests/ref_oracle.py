@@ -1,4 +1,4 @@
-"""Runs pieces of the UNMODIFIED reference (installed in baseline/_ref) as an oracle. Executed in a SUBPROCESS by
+"""Runs pieces of the UNMODIFIED reference (installed in oracle/_ref) as an oracle. Executed in a SUBPROCESS by
 tests/test_reference_parity.py because the reference's top-level package names (datasets, models, tools, ...) must
 not leak into the test process.   python tests/ref_oracle.py <case> <in.pt> <out.pt>"""
 import logging
@@ -8,7 +8,7 @@ import sys
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.path.join(ROOT, "baseline", "_ref")
+REF = os.path.join(ROOT, "oracle", "_ref")
 sys.path.insert(0, REF)
 logging.disable(logging.CRITICAL)
 
@@ -123,11 +123,12 @@ def main():
         out = {"thetas": thetas}
     elif case == "swin_forward":
         from models.swin_transformer import SwinTransformer
-        torch.manual_seed(d["seed"])
         net = SwinTransformer(img_size=d["img"], embed_dim=d["dim"], depths=d["depths"], num_heads=d["heads"],
                               window_size=d["ws"], num_classes=d["classes"], drop_path_rate=0.0).eval()
+        missing, unexpected = net.load_state_dict(d["state"], strict=False)     # this engine's weights, same keys
         with torch.no_grad():
-            out = {"state": net.state_dict(), "feat": net.forward_features(d["x"]), "logits": net(d["x"])}
+            out = {"missing": list(missing), "unexpected": list(unexpected), "feat": net.forward_features(d["x"]),
+                   "logits": net(d["x"])}
     elif case == "schedule":
         from datasets.datasets_pipeline import ReIDTaskPipeline
         out = {}

@@ -45,7 +45,7 @@ def test_bench_cpu_debug_prints_the_driver_contract():
 
 
 def test_reference_arm_reports_itself_when_the_reference_is_missing(tmp_path):
-    """``--impl reference`` without ``baseline/_ref`` must print ``{"impl": "reference", "unavailable": ...}`` and exit
+    """``--impl reference`` without ``oracle/_ref`` must print ``{"impl": "reference", "unavailable": ...}`` and exit
     0 (driver contract). Checked on the arm's own function with the reference directory pointed elsewhere."""
     sys.path.insert(0, ROOT)
     from baseline import reference_arm as ra
@@ -61,11 +61,11 @@ def test_reference_arm_reports_itself_when_the_reference_is_missing(tmp_path):
 
 
 def test_reference_arm_runs_the_installed_reference():
-    """``--impl reference --cpu-debug``: the unmodified reference in ``baseline/_ref`` driven through its own builder /
+    """``--impl reference --cpu-debug``: the unmodified reference in ``oracle/_ref`` driven through its own builder /
     ``ExperimentStage._process_one_round`` prints the same JSON line (``impl: reference``)."""
     import pytest
-    if not os.path.isdir(os.path.join(ROOT, "baseline", "_ref", "methods")):
-        pytest.skip("reference is not installed in baseline/_ref")
+    if not os.path.isdir(os.path.join(ROOT, "oracle", "_ref", "methods")):
+        pytest.skip("the reference oracle is not built in oracle/_ref")
     d = _run("--impl", "reference", "--cpu-debug", "--steps", "1", "--warmup", "1")
     assert d.get("impl") == "reference" and "unavailable" not in d
     for key in ("metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step", "higher_is_better", "config"):

@@ -1,4 +1,4 @@
-"""Whole-experiment golden parity (SURVEY §7.4): the UNMODIFIED reference (``baseline/_ref``, subprocess) and this engine
+"""Whole-experiment golden parity (SURVEY §7.4): the UNMODIFIED reference (``oracle/_ref``, subprocess) and this engine
 run the same tiny fp32 CPU experiment – same initial weights, same synthetic splits, every split smaller than one batch
 so the reference's shuffling cannot change the arithmetic – and every payload / model checkpoint the reference wrote is
 compared tensor by tensor with the file this engine wrote under the same name."""
@@ -15,13 +15,12 @@ from flpr_b200.runtime.config import merge_experiment
 from flpr_b200.runtime.experiment import ExperimentStage
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.path.join(ROOT, "baseline", "_ref")
+REF = os.path.join(ROOT, "oracle", "_ref")
 pytestmark = pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "methods")),
-                                reason="reference is not installed in baseline/_ref")
+                                reason="the reference oracle is not built in oracle/_ref")
 
 H, W, CLIENTS, TASKS, ROUNDS = 32, 16, 2, 2, 2
-# The default run keeps the suite around ten minutes on a CPU box; FLPR_GOLDEN_FULL=1 adds the remaining variants
-# (last full run: profiles/golden_parity.md).
+# The default run keeps the suite around ten minutes on a CPU box; FLPR_GOLDEN_FULL=1 adds the remaining variants.
 OVERRIDES: dict = {}        # per-test overrides of the shared config (epochs, lr); see test_early_stopping_...
 full = pytest.mark.skipif(os.environ.get("FLPR_GOLDEN_FULL") != "1", reason="set FLPR_GOLDEN_FULL=1 for the full matrix")
 

@@ -145,7 +145,7 @@ def test_experiment_with_concurrent_client_streams(tmp_path, method):
 
 @pytest.mark.parametrize("name,size", [("resnet50", (256, 128)), ("resnet18", (128, 64))])
 def test_native_trunk_matches_library_trunk(name, size):
-    """Frozen trunk on the tcgen05 implicit-GEMM kernels (incl. the stride-2 convolutions) vs the cuDNN path."""
+    """Frozen trunk on the wgmma implicit-GEMM kernels (incl. the stride-2 convolutions) vs the cuDNN path."""
     from flpr_b200.models import resnet as R
     from flpr_b200.models.frozen import FoldedTrunk
     from flpr_b200.ops import native
@@ -323,7 +323,7 @@ def test_fedavg_training_step_launches_no_library_conv_or_batchnorm(tmp_path):
     bad = [n for n in names if any(t in n.lower() for t in ("cudnn", "cutlass", "batch_norm", "implicit_gemm",
                                                              "sgemm", "gemv", "cublas", "xmma"))]
     assert not bad, bad
-    assert any("tcgen05" in n for n in names), names[:20]
+    assert any("wgmma" in n for n in names), names[:20]
 
 
 def test_mapped_checkpoint_store_dma_into_registered_files():
@@ -385,9 +385,9 @@ def test_peer_memory_collectives_on_two_or_more_gpus():
 
 
 def test_swin_head_step_runs_its_linears_on_tcgen05():
-    """BASELINE config 4 (FedSTIL over Swin-T, bf16): every Linear of the trainable stage and the classifier runs on the
-    tcgen05 GEMM (forward, dgrad, wgrad into the arena slot) - no cuBLAS / cuBLASLt kernel in a head step - and the step
-    agrees with the fp32 module."""
+    """(Name kept from the Blackwell version of the kernel.) BASELINE config 4 (FedSTIL over Swin-T, bf16): every Linear
+    of the trainable stage and the classifier runs on the wgmma GEMM (forward, dgrad, wgrad into the arena slot) - no
+    cuBLAS / cuBLASLt kernel in a head step - and the step agrees with the fp32 module."""
     import copy as _copy
     from torch.profiler import ProfilerActivity, profile
     from flpr_b200.models.swin import TcLinear
@@ -428,4 +428,4 @@ def test_swin_head_step_runs_its_linears_on_tcgen05():
     names = [e.key for e in prof.key_averages()]
     bad = [n for n in names if any(t in n.lower() for t in ("cublas", "cutlass", "gemv", "sgemm", "xmma", "nvjet"))]
     assert not bad, bad
-    assert any("tcgen05" in n for n in names)
+    assert any("wgmma" in n for n in names)

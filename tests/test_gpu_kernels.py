@@ -1,4 +1,4 @@
-"""Numerics of every sm_100a kernel against a plain fp32 PyTorch reference (runs on the B200 box)."""
+"""Numerics of every sm_90a kernel against a plain fp32 PyTorch reference (runs on a GPU box)."""
 import math
 
 import pytest
@@ -7,17 +7,20 @@ import torch
 pytestmark = pytest.mark.gpu
 
 
-@pytest.fixture(autouse=True, params=["persistent", "classic", "pair"])
+@pytest.fixture(autouse=True, params=["persistent", "classic", "pair", "generic-epilogue"])
 def gemm_kernel_variant(request):
-    """Every test runs against the tcgen05 GEMM kernels: persistent (default), one-tile-per-CTA, and the CTA-pair
-    (cta_group::2) kernel on the shapes it covers."""
+    """Every test runs against the wgmma GEMM kernel: persistent grid (default), one CTA per tile, the CTA-pair kernel
+    (2-CTA clusters sharing the B tile through TMA multicast) on the shapes it covers, and the generic epilogue forced
+    on the shapes that would take the lean one."""
     from flpr_b200.ops import native
     lib = native.load()
     lib.flpr_gemm_set_persistent(0 if request.param == "classic" else 1)
     lib.flpr_gemm_set_pair(1 if request.param == "pair" else 0)       # "persistent" = single-CTA persistent kernel
+    lib.flpr_gemm_set_generic_epilogue(1 if request.param == "generic-epilogue" else 0)
     yield request.param
     lib.flpr_gemm_set_persistent(1)
     lib.flpr_gemm_set_pair(-1)
+    lib.flpr_gemm_set_generic_epilogue(-1)
 
 
 def _ref_gemm(a, b):
@@ -589,7 +592,7 @@ def test_fused_window_attention(dtype, bw, n, h, d, nwb):
 @pytest.mark.parametrize("hard", [False, True])
 @pytest.mark.parametrize("margin", [0.3, None])
 def test_fused_triplet_loss_matches_tensor_ops(cosine, hard, margin):
-    """Triplet loss with the Gram matrix on the tcgen05 GEMM and fused mining (``csrc/loss_ops.cu``), forward and the
+    """Triplet loss with the Gram matrix on the wgmma GEMM and fused mining (``csrc/loss_ops.cu``), forward and the
     gradient w.r.t. the features, against the plain fp32 tensor-op form (``criterions/triplet_loss.py:89-127``)."""
     from flpr_b200.criterions import TripletLoss
     torch.manual_seed(3)
@@ -644,7 +647,7 @@ def test_fused_kd_and_bce_distill(dtype):
 
 @pytest.mark.parametrize("bw,n,h,nwb", [(64 * 64, 49, 3, 64), (64 * 16, 49, 6, 16), (64, 49, 24, 1), (37, 16, 12, 1)])
 def test_window_attention_tcgen05_forward(bw, n, h, nwb):
-    """The tcgen05 forward (QK^T and PV on the tensor cores, TMEM accumulators, thread-per-row softmax) against the
+    """(Name kept from the Blackwell version of the kernel.) The wgmma forward (QK^T and PV on the tensor cores, register accumulators, quad-per-row softmax) against the
     CUDA-core kernel and the fp32 tensor-op reference, at the real Swin-T stage shapes (batch 64)."""
     from flpr_b200.ops import native
     from flpr_b200.ops.fused import window_attention

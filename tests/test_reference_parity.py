@@ -1,5 +1,8 @@
-"""Golden parity against the UNMODIFIED reference (baseline/_ref, run in a subprocess as an oracle): ranking metrics,
-distances, losses, FedAvg aggregation (incl. stale clients) and the FedSTIL spatial-temporal mix."""
+"""Golden parity against the UNMODIFIED reference: ranking metrics, distances, losses, FedAvg aggregation (incl. stale
+clients) and the FedSTIL spatial-temporal mix. The reference's answers are stored under ``tests/golden/reference_parity``
+(one file per test and oracle case, recorded by running ``tests/ref_oracle.py`` against the reference installed in
+``oracle/_ref`` with ``FLPR_RECORD_GOLDEN=1``); every run compares this engine with them."""
+import hashlib
 import os
 import subprocess
 import sys
@@ -8,19 +11,30 @@ import pytest
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.path.join(ROOT, "baseline", "_ref")
-pytestmark = pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "methods")),
-                                reason="reference is not installed in baseline/_ref")
+REF = os.path.join(ROOT, "oracle", "_ref")
+GOLDEN = os.path.join(ROOT, "tests", "golden", "reference_parity")
+
+
+def _golden_path(case):
+    test = os.environ["PYTEST_CURRENT_TEST"].split(" ")[0].split("::", 1)[1]
+    return os.path.join(GOLDEN, f"{hashlib.sha1(test.encode()).hexdigest()[:12]}_{case}.pt")
 
 
 def oracle(case, payload, tmp_path):
+    golden = _golden_path(case)
+    if os.environ.get("FLPR_RECORD_GOLDEN") != "1":
+        assert os.path.exists(golden), f"no stored reference answer {golden} (record it with FLPR_RECORD_GOLDEN=1)"
+        return torch.load(golden, weights_only=False)
     inp, outp = str(tmp_path / f"{case}_in.pt"), str(tmp_path / f"{case}_out.pt")
     torch.save(payload, inp)
     env = dict(os.environ, TORCH_FORCE_NO_WEIGHTS_ONLY_LOAD="1")
     r = subprocess.run([sys.executable, os.path.join(ROOT, "tests", "ref_oracle.py"), case, inp, outp],
                        capture_output=True, text=True, env=env, timeout=600)
     assert r.returncode == 0, r.stderr[-2000:]
-    return torch.load(outp, weights_only=False)
+    out = torch.load(outp, weights_only=False)
+    os.makedirs(GOLDEN, exist_ok=True)
+    torch.save(out, golden)
+    return out
 
 
 def test_ranking_metrics_match_reference(tmp_path):
@@ -232,13 +246,14 @@ def test_swin_transformer_matches_reference(tmp_path):
     fused-attention code path (tensor-op form on CPU) and the SDPA path (shifted windows, masks, patch merging)."""
     from flpr_b200.models.swin import SwinTransformer, WindowAttention
     torch.manual_seed(5)
-    cfg = {"img": 56, "dim": 24, "depths": (2, 2), "heads": (2, 4), "ws": 7, "classes": 5, "seed": 7,
-           "x": torch.randn(2, 3, 56, 56)}
-    ref = oracle("swin_forward", cfg, tmp_path)
     net = SwinTransformer(img_size=56, embed_dim=24, depths=(2, 2), num_heads=(2, 4), window_size=7, num_classes=5,
                           drop_path_rate=0.0).eval()
-    missing, unexpected = net.load_state_dict(ref["state"], strict=False)
-    assert not [k for k in missing if "relative_position_index" not in k and "attn_mask" not in k], missing
+    cfg = {"img": 56, "dim": 24, "depths": (2, 2), "heads": (2, 4), "ws": 7, "classes": 5,
+           "x": torch.randn(2, 3, 56, 56), "state": net.state_dict()}
+    ref = oracle("swin_forward", cfg, tmp_path)
+    # the reference module takes this engine's state dict: every parameter / buffer key exists on both sides
+    assert not [k for k in ref["missing"] if "relative_position_index" not in k and "attn_mask" not in k], ref["missing"]
+    assert not [k for k in ref["unexpected"] if not k.endswith(("relative_position_index", "attn_mask"))], ref["unexpected"]
     for fused in (True, False):
         for m in net.modules():
             if isinstance(m, WindowAttention):
