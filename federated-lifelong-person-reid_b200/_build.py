@@ -19,7 +19,7 @@ OBJ_DIR = os.path.join(PKG_DIR, "build")
 LIB_PATH = os.path.join(LIB_DIR, "libflpr_b200.so")
 STAMP = os.path.join(LIB_DIR, "build.stamp")
 
-CUDA_SOURCES = ["gemm_wgmma.cu", "fedcomm.cu", "fused_ops.cu", "loss_ops.cu", "layer_ops.cu"]
+CUDA_SOURCES = ["gemm_wgmma.cu", "fedcomm.cu", "fused_ops.cu", "loss_ops.cu", "layer_ops.cu", "rerank.cu"]
 CXX_SOURCES = ["runtime.cpp"]
 
 NVCC_FLAGS = [

@@ -85,3 +85,21 @@ def write_imagefolder_tree(datasets_dir: str, tasks: Sequence[str], num_ids: int
                 Image.fromarray(img.numpy()).save(os.path.join(d, f"{k:04d}.jpg"), quality=95)
             out[task] = ds.person_ids
     return out
+
+
+def clustered_features(num_query: int, num_gallery: int, dim: int, num_ids: int, seed: int = 0, spread: float = 0.6,
+                       device="cpu"):
+    """Seeded synthetic ReID embeddings: one random unit centre per identity, every image its identity's centre plus
+    isotropic noise (``spread`` = noise norm relative to the centre), L2-normalised. Query and gallery identities are
+    drawn independently and uniformly from ``num_ids``. Returns ``(query [Q, dim], q_labels, gallery [G, dim],
+    g_labels)`` as fp32 / int64 tensors on ``device``. (Used by the re-ranking tests and ``scripts/rerank_bench.py``.)"""
+    g = torch.Generator().manual_seed(seed)
+    centres = torch.nn.functional.normalize(torch.randn(num_ids, dim, generator=g), dim=1)
+
+    def draw(n):
+        lab = torch.randint(0, num_ids, (n,), generator=g)
+        x = centres[lab] + spread * torch.randn(n, dim, generator=g) / dim ** 0.5
+        return torch.nn.functional.normalize(x, dim=1).to(device), lab.to(device)
+    q, ql = draw(num_query)
+    gf, gl = draw(num_gallery)
+    return q, ql, gf, gl

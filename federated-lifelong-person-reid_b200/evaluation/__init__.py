@@ -1,6 +1,6 @@
-"""Evaluation entry points (``tools/evaluate.py``): CMC / mAP on device."""
+"""Evaluation entry points (``tools/evaluate.py``): CMC / mAP on device, optionally after k-reciprocal re-ranking."""
 from ..ops.rank import (evaluate, evaluate_sharded, rank_metrics, rank_metrics_reference,  # noqa: F401
-                        similarity)
+                        re_ranking, re_ranking_reference, similarity)
 from .sharded import ShardedRanker  # noqa: F401
 
 

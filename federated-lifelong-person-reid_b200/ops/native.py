@@ -68,6 +68,13 @@ def _signatures() -> dict:
         "flpr_gap_fwd": [P, P, P, I, I, I, P],
         "flpr_gap_bwd": [P, P, I, I, I, P],
         "flpr_rank_eval": [P, P, P, P, P, I, I, L, P],
+        "flpr_rr_sqnorm": [P, P, I, I, L, P],
+        "flpr_rr_distance": [P, P, I, L, P],
+        "flpr_rr_topk": [P, P, I, I, L, P],
+        "flpr_rr_encode": [P, P, P, P, P, I, I, I, I, L, P],
+        "flpr_rr_expand": [P, P, P, P, P, P, P, I, I, I, I, I, P],
+        "flpr_rr_index": [P, P, P, I, I, I, I, P, P, P, P, P],
+        "flpr_rr_jaccard": [P, P, P, I, P, P, P, P, L, P, I, I, I, F, P],
         "flpr_augment_u8": [P, P, P, I, I, I, P, P, F, F, F, F, F, F, I, P],
         "flpr_herding": [P, P, P, P, I, I, I, I, P],
         "flpr_window_attn_fwd": [P, P, P, I, I, I, I, I, F, I, P],

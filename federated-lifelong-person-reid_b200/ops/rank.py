@@ -5,7 +5,7 @@ numpy set ops per query) with two kernel launches and a single device->host copy
 """
 from __future__ import annotations
 
-from typing import Tuple
+from typing import Dict, NamedTuple, Optional, Tuple
 
 import numpy as np
 import torch
@@ -121,13 +121,20 @@ def rank_metrics_with_cameras(sim: torch.Tensor, q_labels: torch.Tensor, g_label
 def evaluate(query_features: torch.Tensor, query_labels: torch.Tensor, gallery_features: torch.Tensor,
              gallery_labels: torch.Tensor, query_camera_labels: torch.Tensor | None = None,
              gallery_camera_labels: torch.Tensor | None = None, device: str | torch.device | None = None,
-             precise: bool = True) -> Tuple[np.ndarray, float]:
+             precise: bool = True, re_ranking: Optional[Dict] = None) -> Tuple[np.ndarray, float]:
     """Drop-in for ``tools.evaluate.evaluate`` (same positional order). Camera labels are optional - the reference's
-    runtime never passes them - and switch on its same-camera / mis-detection junk rule."""
+    runtime never passes them - and switch on its same-camera / mis-detection junk rule.
+
+    ``re_ranking``: ``None`` (plain ranking) or a dict of :func:`re_ranking`'s ``k1`` / ``k2`` / ``lambda_value``
+    (missing keys take the defaults); the queries are then ranked by the negated re-ranked distance."""
     if device is not None:
         query_features = query_features.to(device)
         gallery_features = gallery_features.to(device)
-    sim = similarity(query_features, gallery_features, precise=precise)
+    rr = re_ranking_params(re_ranking)
+    if rr is not None:
+        sim = -_re_ranking(query_features, gallery_features, **rr)
+    else:
+        sim = similarity(query_features, gallery_features, precise=precise)
     if query_camera_labels is not None and gallery_camera_labels is not None:
         return rank_metrics_with_cameras(sim, query_labels, gallery_labels, query_camera_labels,
                                          gallery_camera_labels)
@@ -212,3 +219,262 @@ def evaluate_sharded(query_features: torch.Tensor, query_labels: torch.Tensor, g
     m_ap = (ap * has).sum() / nq
     out = torch.cat([cmc, m_ap.view(1)]).cpu().numpy()
     return out[:-1], float(out[-1])
+
+
+# ------------------------------------------------------------------------------------------------- k-reciprocal re-ranking
+RE_RANKING_DEFAULTS = {"k1": 20, "k2": 6, "lambda_value": 0.3}
+
+
+def _is_int(v) -> bool:
+    return isinstance(v, (int, np.integer)) and not isinstance(v, bool)
+
+
+def check_re_ranking_params(k1, k2, lambda_value) -> Tuple[int, int, float]:
+    """``1 <= k1 <= 63`` (a row's ``k1 + 1`` neighbours fit two per lane of one warp), ``1 <= k2 <= k1 + 1``,
+    ``0 <= lambda_value <= 1``; anything else raises ``ValueError``."""
+    if not _is_int(k1) or not 1 <= k1 <= 63:
+        raise ValueError(f"re-ranking k1 must be an integer in [1, 63], got {k1!r}")
+    if not _is_int(k2) or not 1 <= k2 <= k1 + 1:
+        raise ValueError(f"re-ranking k2 must be an integer in [1, k1 + 1 = {k1 + 1}], got {k2!r}")
+    if isinstance(lambda_value, bool) or not isinstance(lambda_value, (int, float, np.floating)) \
+            or not 0.0 <= float(lambda_value) <= 1.0:
+        raise ValueError(f"re-ranking lambda_value must be a number in [0, 1], got {lambda_value!r}")
+    return int(k1), int(k2), float(lambda_value)
+
+
+def re_ranking_params(spec) -> Optional[Dict]:
+    """``engine_opts.re_ranking`` / ``evaluate(re_ranking=...)`` -> ``None`` (off) or a full, checked parameter dict.
+    ``False`` / ``None``: off; ``True``: the defaults; a dict: its keys over the defaults."""
+    if spec is None or spec is False:
+        return None
+    if spec is True:
+        spec = {}
+    if not isinstance(spec, dict):
+        raise ValueError(f"re_ranking must be false, true or a dict of k1 / k2 / lambda_value, got {spec!r}")
+    unknown = set(spec) - set(RE_RANKING_DEFAULTS)
+    if unknown:
+        raise ValueError(f"unknown re_ranking parameters {sorted(unknown)} (known: k1, k2, lambda_value)")
+    p = dict(RE_RANKING_DEFAULTS, **spec)
+    k1, k2, lam = check_re_ranking_params(p["k1"], p["k2"], p["lambda_value"])
+    return {"k1": k1, "k2": k2, "lambda_value": lam}
+
+
+def _expansion_h(k1: int) -> int:
+    return int(round(k1 / 2)) + 1          # Python's round: half to even
+
+
+# ---- float64 reference (the test oracle; also what CPU tensors run) ------------------------------------------------------
+def re_ranking_distance_reference(query: torch.Tensor, gallery: torch.Tensor) -> torch.Tensor:
+    """Step 1 in float64 on the inputs' device: squared euclidean distances of ``X = cat(query, gallery)``, clamped at 0,
+    zero diagonal, every row divided by its maximum (an all-zero row stays zero)."""
+    x = torch.cat([query, gallery]).double()
+    sq = (x * x).sum(1)
+    d = (sq.view(-1, 1) + sq.view(1, -1) - 2.0 * (x @ x.t())).clamp_min(0.0)
+    d.fill_diagonal_(0.0)
+    mx = d.max(1, keepdim=True).values
+    return torch.where(mx > 0, d / torch.where(mx > 0, mx, torch.ones_like(mx)), d)
+
+
+def re_ranking_topk_reference(D: torch.Tensor, k1: int, rows=None, chunk: int = 1024) -> torch.Tensor:
+    """Step 2: ``R[i, :K]``, ``K = min(k1 + 1, N)``: stable ascending sort of ``D[i]`` (ties to the lower index).
+    ``rows``: only these rows (int64 ``[len(rows), K]``), else all. Runs on ``D``'s device, chunked."""
+    n = D.shape[0]
+    k = min(k1 + 1, n)
+    rows = torch.arange(n, device=D.device) if rows is None else torch.as_tensor(rows, device=D.device).long()
+    out = []
+    for s in range(0, len(rows), chunk):
+        blk = D[rows[s:s + chunk]].double()
+        out.append(torch.sort(blk, dim=1, stable=True).indices[:, :k])
+    return torch.cat(out) if out else torch.zeros(0, k, dtype=torch.long, device=D.device)
+
+
+def re_ranking_encode_reference(d_row, R: np.ndarray, i: int, k1: int):
+    """Steps 3-5 for row ``i`` alone: ``(K(i), E(i), weights)``. ``d_row``: ``D[i, :]``; ``R``: the full initial ranking
+    (int numpy ``[N, K]``). ``K(i)`` is in ``R[i]``'s order, ``E(i)`` ascending, ``weights`` float64 over ``E(i)``."""
+    R = np.asarray(R)
+    K = R.shape[1]
+    h = min(_expansion_h(k1), K)
+    F = R[i, :K]
+    Ki = F[(R[F, :K] == i).any(1)]
+    E = [int(v) for v in Ki]
+    for c in Ki:
+        fw = R[c, :h]
+        Kc = fw[(R[fw, :h] == c).any(1)]
+        inter = int(np.isin(Kc, Ki).sum())
+        if 3 * inter > 2 * len(Kc):                     # |Kc n K(i)| > (2/3) |Kc|
+            E.extend(int(v) for v in Kc)
+    E = np.array(sorted(set(E)), dtype=np.int64)
+    d = torch.as_tensor(d_row).double().cpu().numpy()
+    w = np.exp(-d[E])
+    if len(E):
+        w = w / w.sum()
+    return [int(v) for v in Ki], E, w
+
+
+def re_ranking_reference(query: torch.Tensor, gallery: torch.Tensor, k1: int = 20, k2: int = 6,
+                         lambda_value: float = 0.3, distance: Optional[torch.Tensor] = None, details: bool = False):
+    """k-reciprocal re-ranking, a plain float64 transcription of the eight steps (DESIGN §3). Returns the ``[Q, G]``
+    float64 distance on the inputs' device; ``distance``: start from this ``D`` (step 1 skipped). ``details``: also a
+    dict of the intermediates ``D, R, K, E, V, Vq`` (dense ``V`` / ``Vq``, lists of index arrays ``K`` / ``E``)."""
+    k1, k2, lambda_value = check_re_ranking_params(k1, k2, lambda_value)
+    nq = query.shape[0]
+    D = re_ranking_distance_reference(query, gallery) if distance is None else distance.double()
+    dev = D.device
+    n = D.shape[0]
+    R = re_ranking_topk_reference(D, k1).cpu().numpy()
+    Dc = D.cpu().numpy()
+    V = np.zeros((n, n), dtype=np.float64)
+    Ks, Es = [], []
+    for i in range(n):
+        Ki, Ei, w = re_ranking_encode_reference(Dc[i], R, i, k1)
+        V[i, Ei] = w
+        Ks.append(Ki)
+        Es.append(Ei)
+    Vt = torch.from_numpy(V).to(dev)
+    if k2 != 1:                                            # local query expansion: mean over R[i, :k2] (clamped)
+        kk = min(k2, R.shape[1])
+        Rt = torch.from_numpy(R[:, :kk]).to(dev)
+        Vq = torch.zeros_like(Vt)
+        for r in range(kk):
+            Vq += Vt[Rt[:, r]]
+        Vq /= kk
+    else:
+        Vq = Vt
+    final = torch.empty(nq, n - nq, dtype=torch.float64, device=dev)
+    Vg = Vq[nq:]
+    for i in range(nq):
+        nz = torch.nonzero(Vq[i]).flatten()
+        m = torch.minimum(Vq[i, nz].view(1, -1), Vg[:, nz]).sum(1)
+        final[i] = 1.0 - m / (2.0 - m)
+    final = (1.0 - lambda_value) * final + lambda_value * D[:nq, nq:]
+    if details:
+        return final, {"D": D, "R": R, "K": Ks, "E": Es, "V": V, "Vq": Vq.cpu().numpy()}
+    return final
+
+
+# ---- native stages -------------------------------------------------------------------------------------------------------
+class SparseRows(NamedTuple):
+    """Fixed-capacity sparse rows: row ``i`` holds ``nnz[i]`` entries ``cols[i, :nnz[i]]`` (ascending) / ``vals``."""
+    cols: torch.Tensor     # int32 [N, cap]
+    vals: torch.Tensor     # fp32  [N, cap]
+    nnz: torch.Tensor      # int32 [N]
+
+    def dense(self, n: int) -> torch.Tensor:
+        out = torch.zeros(self.cols.shape[0], n, dtype=torch.float64, device=self.cols.device)
+        cap = self.cols.shape[1]
+        mask = torch.arange(cap, device=self.cols.device).view(1, -1) < self.nnz.view(-1, 1).long()
+        r = torch.arange(self.cols.shape[0], device=self.cols.device).view(-1, 1).expand(-1, cap)
+        out[r[mask], self.cols.long()[mask]] = self.vals.double()[mask]
+        return out
+
+
+def _rr_call(name: str, *args) -> None:
+    lib = native.kernels()
+    native.check(getattr(lib, name)(*args), name)
+    native.count_launch()
+
+
+def rr_distance(S: torch.Tensor, x: torch.Tensor) -> torch.Tensor:
+    """Step 1 on the kernels: ``S = x x^T`` (fp32 ``[N, N]``, contiguous) becomes ``D`` in place; ``x``: the features."""
+    x = x.float().contiguous()
+    n = x.shape[0]
+    sqn = torch.empty(n, dtype=torch.float32, device=x.device)
+    st = native.stream_of(x.device)
+    _rr_call("flpr_rr_sqnorm", native.ptr(x), native.ptr(sqn), n, x.shape[1], x.stride(0), st)
+    _rr_call("flpr_rr_distance", native.ptr(S), native.ptr(sqn), n, S.stride(0), st)
+    return S
+
+
+def rr_topk(D: torch.Tensor, k1: int) -> torch.Tensor:
+    """Step 2: int32 ``[N, min(k1 + 1, N)]``."""
+    n = D.shape[0]
+    k = min(k1 + 1, n)
+    R = torch.empty(n, k, dtype=torch.int32, device=D.device)
+    _rr_call("flpr_rr_topk", native.ptr(D), native.ptr(R), n, k, D.stride(0), native.stream_of(D.device))
+    return R
+
+
+def rr_encode(D: torch.Tensor, R: torch.Tensor, k1: int) -> SparseRows:
+    """Steps 3-5: the weighted k-reciprocal expansion of every row (capacity ``K (h + 1)``)."""
+    n, k = R.shape
+    hh = min(_expansion_h(k1), k)
+    cap = k * (hh + 1)
+    cols = torch.zeros(n, cap, dtype=torch.int32, device=D.device)
+    vals = torch.zeros(n, cap, dtype=torch.float32, device=D.device)
+    nnz = torch.empty(n, dtype=torch.int32, device=D.device)
+    _rr_call("flpr_rr_encode", native.ptr(D), native.ptr(R), native.ptr(cols), native.ptr(vals), native.ptr(nnz), n, k,
+             hh, cap, D.stride(0), native.stream_of(D.device))
+    return SparseRows(cols, vals, nnz)
+
+
+def rr_expand(V: SparseRows, R: torch.Tensor, k2: int) -> SparseRows:
+    """Step 6: ``V'_i = mean_{r < k2} V_{R[i, r]}`` (``k2`` clamped to ``R``'s width); ``k2 == 1`` returns ``V``."""
+    if k2 == 1:
+        return V
+    n, k = R.shape
+    k2 = min(k2, k)
+    cap = V.cols.shape[1]
+    ocap = k2 * cap
+    cols = torch.zeros(n, ocap, dtype=torch.int32, device=R.device)
+    vals = torch.zeros(n, ocap, dtype=torch.float32, device=R.device)
+    nnz = torch.empty(n, dtype=torch.int32, device=R.device)
+    _rr_call("flpr_rr_expand", native.ptr(V.cols), native.ptr(V.vals), native.ptr(V.nnz), native.ptr(R),
+             native.ptr(cols), native.ptr(vals), native.ptr(nnz), n, k, k2, cap, ocap, native.stream_of(R.device))
+    return SparseRows(cols, vals, nnz)
+
+
+def rr_index(Vq: SparseRows, num_query: int):
+    """Inverted index of the gallery rows of ``V'``: ``(off [N + 1], row [E], val [E])``; the entries of column ``j``
+    are ``off[j] .. off[j + 1]`` (gallery rows numbered from 0)."""
+    n, cap = Vq.cols.shape
+    g = n - num_query
+    dev = Vq.cols.device
+    total = int(Vq.nnz[num_query:].sum()) if g > 0 else 0
+    cnt = torch.empty(n, dtype=torch.int32, device=dev)
+    off = torch.empty(n + 1, dtype=torch.int32, device=dev)
+    rows = torch.empty(max(total, 1), dtype=torch.int32, device=dev)
+    vals = torch.empty(max(total, 1), dtype=torch.float32, device=dev)
+    _rr_call("flpr_rr_index", native.ptr(Vq.cols), native.ptr(Vq.vals), native.ptr(Vq.nnz), num_query, g, n, cap,
+             native.ptr(cnt), native.ptr(off), native.ptr(rows), native.ptr(vals), native.stream_of(dev))
+    return off, rows, vals
+
+
+def rr_jaccard(Vq: SparseRows, D: torch.Tensor, num_query: int, lambda_value: float, tile: int = 0) -> torch.Tensor:
+    """Steps 7-8: ``[Q, G]`` fp32 ``(1 - lambda) J + lambda D[:Q, Q:]``. ``tile``: gallery items per block (0 = as many
+    as fit in shared memory)."""
+    n = D.shape[0]
+    g = n - num_query
+    off, rows, vals = rr_index(Vq, num_query)
+    out = torch.empty(num_query, g, dtype=torch.float32, device=D.device)
+    _rr_call("flpr_rr_jaccard", native.ptr(Vq.cols), native.ptr(Vq.vals), native.ptr(Vq.nnz), Vq.cols.shape[1],
+             native.ptr(off), native.ptr(rows), native.ptr(vals), native.ptr(D), D.stride(0), native.ptr(out),
+             num_query, g, int(tile), float(lambda_value), native.stream_of(D.device))
+    return out
+
+
+def re_ranking_from_distance(D: torch.Tensor, num_query: int, k1: int = 20, k2: int = 6, lambda_value: float = 0.3,
+                             tile: int = 0) -> torch.Tensor:
+    """Steps 2-8 on the kernels, from a given fp32 ``D`` (``[N, N]``, contiguous, as :func:`rr_distance` leaves it)."""
+    k1, k2, lambda_value = check_re_ranking_params(k1, k2, lambda_value)
+    R = rr_topk(D, k1)
+    V = rr_encode(D, R, k1)
+    Vq = rr_expand(V, R, k2)
+    return rr_jaccard(Vq, D, num_query, lambda_value, tile)
+
+
+def re_ranking(query: torch.Tensor, gallery: torch.Tensor, k1: int = 20, k2: int = 6,
+               lambda_value: float = 0.3) -> torch.Tensor:
+    """k-reciprocal re-ranking (Zhong et al., CVPR 2017): ``[Q, G]`` fp32 distance, smaller = more similar.
+
+    CUDA tensors: the similarity GEMM of :func:`similarity` (hi/lo split, ~fp32) and the stages of ``csrc/rerank.cu``;
+    memory is about ``4 N^2`` bytes for ``D`` plus ``O(N k2 cap)`` for the sparse rows (``N = Q + G``). CPU tensors:
+    :func:`re_ranking_reference` in float64, returned as fp32."""
+    k1, k2, lambda_value = check_re_ranking_params(k1, k2, lambda_value)
+    if not native.on_device(query, "flpr_rr_topk"):
+        return re_ranking_reference(query, gallery, k1, k2, lambda_value).float()
+    x = torch.cat([query, gallery]).float().contiguous()
+    D = rr_distance(similarity(x, x, precise=True).contiguous(), x)
+    return re_ranking_from_distance(D, query.shape[0], k1, k2, lambda_value)
+
+
+_re_ranking = re_ranking

@@ -21,6 +21,7 @@ from ..criterions import criterions
 from ..data.pipeline import ReIDTaskPipeline
 from ..methods import methods
 from ..models import nets, optimizers, schedulers
+from ..ops.rank import re_ranking_params
 from .checkpoint import CheckpointStore
 from .modules import ClientModule, ModelModule, ServerModule
 
@@ -135,6 +136,7 @@ def parser_clients(exp_config: Dict, common_config: Dict, device="cpu", store: O
                                     device_loader=eng.get("device_augment", True), source_factory=source_factory)
         kwargs = {n: p for n, p in client_config.items() if n not in ("client_name",)}
         kwargs.setdefault("reference_compat", eng.get("reference_compat", True))
+        kwargs.setdefault("re_ranking", re_ranking_params(eng.get("re_ranking", False)))
         anchor = eng.get("train_l1_anchor")
         kwargs.setdefault("train_l1_anchor", bool(eng.get("reference_compat", True) if anchor is None else anchor))
         clients.append(methods[exp_config["exp_method"]].Client(

@@ -35,6 +35,8 @@ ENGINE_DEFAULTS: Dict[str, Any] = {
                                       # next to the training kernels)
     "sharded_validation": False,      # world > 1: all ranks rank every client's gallery in 1/world slices
                                       # (evaluation/sharded.py) instead of each rank validating its own clients alone
+    "re_ranking": False,              # also rank with k-reciprocal re-ranking (val_rr_* next to val_*): true = k1 20,
+                                      # k2 6, lambda 0.3, or a dict {k1, k2, lambda_value}; not with sharded_validation
     "client_threads": True,           # `parallel` clients per device train concurrently on their own CUDA streams
     "resume": False,                  # continue from {checkpoints_dir}/{exp}/_resume/rank{r}.ckpt when present
     "resume_interval": 0,             # write the resume manifest every N rounds (0 = never)

@@ -208,6 +208,7 @@ class ExperimentStage:
             self.run_experiment(exp_config)
 
     def run_experiment(self, exp_config: Dict) -> ExperimentLog:
+        self._check_re_ranking(exp_config)
         same_seeds(exp_config["random_seed"])
         format_time = datetime.now().strftime("%Y-%m-%d-%H-%M")
         log = ExperimentLog(os.path.join(self.common_config["logs_dir"], f"{exp_config['exp_name']}-{format_time}.json"),
@@ -391,6 +392,17 @@ class ExperimentStage:
                 for _ in range(len(cfg["tasks"])):                   # one collective per task of that client
                     ranker.participate(cid % self.world)
 
+    def _check_re_ranking(self, exp_config: Dict) -> None:
+        """``engine_opts.re_ranking`` needs the gallery-to-gallery neighbourhoods of the WHOLE gallery, which the
+        gallery-sharded validation never holds on one rank: refuse the combination instead of skipping re-ranking."""
+        from ..ops.rank import re_ranking_params
+        eng = exp_config["engine_opts"]
+        rr = re_ranking_params(eng.get("re_ranking", False))
+        if rr is not None and eng.get("sharded_validation", False) and self.world > 1:
+            raise ValueError("engine_opts.re_ranking cannot be combined with engine_opts.sharded_validation on "
+                             f"{self.world} ranks: re-ranking needs the neighbourhoods of the whole gallery on one rank. "
+                             "Turn one of the two off.")
+
     def _comm_stream(self):
         st = getattr(self, "_comm_stream_obj", None)
         if st is None:
@@ -493,12 +505,18 @@ class ExperimentStage:
                 pipeline = client.task_pipeline
                 for tid in range(len(pipeline.task_list)):
                     task = pipeline.get_task(tid)
-                    cmc, mAP, _ = client.validate(task_name=task["task_name"], query_loader=task["query_loader"],
-                                                  gallery_loader=task["gallery_loaders"], device=device)
-                    r = lambda k: float(cmc[k]) if len(cmc) > k else float(cmc[-1])  # noqa: E731
-                    log.record(f"data.{client.client_name}.{curr_round}.{task['task_name']}",
-                               {"val_rank_1": r(0), "val_rank_3": r(2), "val_rank_5": r(4), "val_rank_10": r(9),
-                                "val_map": float(mAP)})
+                    out = client.validate(task_name=task["task_name"], query_loader=task["query_loader"],
+                                          gallery_loader=task["gallery_loaders"], device=device)
+                    cmc, mAP = out[0], out[1]
+                    r = lambda c, k: float(c[k]) if len(c) > k else float(c[-1])  # noqa: E731
+                    rec = {"val_rank_1": r(cmc, 0), "val_rank_3": r(cmc, 2), "val_rank_5": r(cmc, 4),
+                           "val_rank_10": r(cmc, 9), "val_map": float(mAP)}
+                    if len(out) > 3:                   # engine_opts.re_ranking: the re-ranked (cmc, mAP)
+                        rr_cmc, rr_map = out[3]
+                        rec.update({"val_rr_rank_1": r(rr_cmc, 0), "val_rr_rank_3": r(rr_cmc, 2),
+                                    "val_rr_rank_5": r(rr_cmc, 4), "val_rr_rank_10": r(rr_cmc, 9),
+                                    "val_rr_map": float(rr_map)})
+                    log.record(f"data.{client.client_name}.{curr_round}.{task['task_name']}", rec)
             except Exception as ex:
                 client.logger.error(ex)
                 raise

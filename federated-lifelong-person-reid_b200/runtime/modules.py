@@ -457,7 +457,15 @@ class ClientModule(_Actor):
         allf = torch.cat([query["features"], gallery["features"]], dim=0)
         avg_rep = allf.sum(dim=0) / max(len(allf), 1)
         self.logger.info_validation(task_name, len(query["features"]), len(gallery["features"]), cmc, mAP)
-        return cmc, mAP, avg_rep
+        rr = getattr(self, "re_ranking", None)
+        if not rr:
+            return cmc, mAP, avg_rep
+        # ``engine_opts.re_ranking``: the same features ranked again by the k-reciprocal distance (ops/rank.py)
+        rr_cmc, rr_map = evaluate(query["features"], query["labels"], gallery["features"], gallery["labels"],
+                                  re_ranking=rr)
+        self.logger.info_validation(task_name, len(query["features"]), len(gallery["features"]), rr_cmc, rr_map,
+                                    label="re-ranked")
+        return cmc, mAP, avg_rep, (rr_cmc, rr_map)
 
     def inference(self, task_name: str, query_loader, gallery_loader, device: str = "cpu", **kwargs) -> Dict:
         """``{query_id: {gallery_id: similarity}}`` as in ``methods/baseline.py:279-303`` (one GEMM, not Q of them)."""

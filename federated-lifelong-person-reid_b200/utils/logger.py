@@ -54,9 +54,11 @@ class Logger:
         parts.append(f"accuracy: {_percent(accuracy)}, loss: {loss:.4f}.")
         self.info("".join(parts))
 
-    def info_validation(self, task_name, query_cnt, gallery_cnt, cmc: Sequence[float], mAP: float) -> None:
+    def info_validation(self, task_name, query_cnt, gallery_cnt, cmc: Sequence[float], mAP: float,
+                        label: str | None = None) -> None:
         at = lambda k: cmc[k - 1] if len(cmc) >= k else cmc[-1]  # noqa: E731  (galleries smaller than ten items)
-        rows = [f"Validation '{task_name}' with {query_cnt:,} query images on {gallery_cnt:,} gallery images:"]
+        head = "Validation" if label is None else f"Validation ({label})"
+        rows = [f"{head} '{task_name}' with {query_cnt:,} query images on {gallery_cnt:,} gallery images:"]
         rows += [f"{_INDENT}|- {label}{_percent(at(k))}" for k, label in _RANKS]
         rows.append(f"{_INDENT}|- mean AP : {_percent(mAP)}")
         rows.append(_INDENT)
