@@ -65,8 +65,8 @@ struct GemmParams {
   int cStride;           // convolution stride (A operand: TMA element strides), 1 or 2
   // persistent scheduling
   int tiles_m, tiles_n, tiles_z, tiles_total;
-  // fused batch-norm statistics: per (m-tile, 32-row quarter) column partials of sum / sum^2 of the fp32 accumulators
-  float* col_part;       // [tiles_m * 4][2][N] or nullptr
+  // fused batch-norm statistics: per (m-tile, 32-row quarter) column partials of sum / sum^2 of the stored output
+  float* col_part;       // [tiles_m * 4][2][N] or nullptr (never together with bias / residual / ReLU)
   int debug;             // FLPR_GEMM_DEBUG bit mask (bottleneck isolation, results are WRONG when set):
                          //   1 skip the epilogue body, 2 skip global stores, 4 skip TMA loads (MMA on stale smem)
 };
@@ -212,8 +212,8 @@ __device__ __forceinline__ void epilogue_chunk(const GemmParams& p, const uint32
   }
   const bool stats_from_stage = p.col_part != nullptr && use_stage && (n0 + c0 + 32 <= p.N);
   if (p.col_part != nullptr && !stats_from_stage) {
-    // fused batch-norm statistics of the raw fp32 conv output (rows >= M are exact zeros: TMA OOB fill)
-    // (of the value that is stored: bf16-rounded when the output is bf16, like the staged path below)
+    // fused batch-norm statistics of alpha * A@B^T as stored: bf16-rounded when the output is bf16, like the staged
+    // path below. col_part excludes bias / residual / ReLU, so rows >= M are exact zeros (TMA OOB fill).
     float s1[32], s2[32];
 #pragma unroll
     for (int j = 0; j < 32; ++j) {
@@ -251,8 +251,12 @@ __device__ __forceinline__ void epilogue_chunk(const GemmParams& p, const uint32
   } else if (row < p.M || use_stage) {
     const long long base = (long long)row * p.ldo + n0 + c0 + tap_off;
     const bool full = (n0 + c0 + 32 <= p.N);
+    // 16-byte vector accesses only where the address itself is 16-byte aligned: `out` and `residual` may be views
+    // that start anywhere (with use_stage, `out` is aligned and ldo % 8 == 0, so this is uniform over the warp)
+    const size_t esz = p.out_bf16 ? 2 : 4;
+    const bool out_vec = ((reinterpret_cast<uintptr_t>(p.out) + (uintptr_t)base * esz) & 15) == 0;
     if (p.residual != nullptr && row < p.M) {
-      if (full && ((base & 7) == 0)) {
+      if (full && ((reinterpret_cast<uintptr_t>(p.residual + base) & 15) == 0)) {
         const uint4* rp = reinterpret_cast<const uint4*>(p.residual + base);
 #pragma unroll
         for (int j4 = 0; j4 < 4; ++j4) {
@@ -282,7 +286,7 @@ __device__ __forceinline__ void epilogue_chunk(const GemmParams& p, const uint32
         if (n0 + c0 + j < p.N) atomicAdd(o + j, v[j]);
     } else if (p.out_bf16) {
       __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.out) + base;
-      if (full && ((base & 7) == 0)) {
+      if (full && out_vec) {
         uint4 pk[4];
 #pragma unroll
         for (int j4 = 0; j4 < 4; ++j4) {
@@ -335,7 +339,7 @@ __device__ __forceinline__ void epilogue_chunk(const GemmParams& p, const uint32
       }
     } else {
       float* o = reinterpret_cast<float*>(p.out) + base;
-      if (full && ((base & 3) == 0)) {
+      if (full && out_vec) {
 #pragma unroll
         for (int j4 = 0; j4 < 8; ++j4)
           reinterpret_cast<float4*>(o)[j4] = make_float4(v[j4 * 4], v[j4 * 4 + 1], v[j4 * 4 + 2], v[j4 * 4 + 3]);
@@ -644,7 +648,8 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
   }
 }
 
-// Deterministic split-K: out[r, c] += sum over s (in order) of part[s][r, c], r < rows, c < cols (row stride ld).
+// Deterministic split-K: out[r, c] = sum over s (in order) of part[s][r, c], r < rows, c < cols (row stride ld).
+// `out` is overwritten, as it is by the single-split kernel.
 __global__ void __launch_bounds__(256) splitk_reduce_kernel(float* out, const float* part, long long rows, long long cols,
                                                            long long ld, long long split_stride, int splits) {
   const long long n = rows * cols;
@@ -653,7 +658,7 @@ __global__ void __launch_bounds__(256) splitk_reduce_kernel(float* out, const fl
     const long long off = r * ld + c;
     float acc = part[off];
     for (int s = 1; s < splits; ++s) acc += part[s * split_stride + off];
-    out[off] += acc;
+    out[off] = acc;
   }
 }
 
@@ -883,7 +888,7 @@ static int dispatch_bn(int BN, int a_mode, int b_mode, const CUtensorMap& ta, co
 }
 
 // Split-K without atomics: the kernel stores the partial product of split s to ws + s * split_stride (plain stores),
-// then splitk_reduce_kernel adds the partials to `out` in split order - the result does not depend on which CTA
+// then splitk_reduce_kernel stores their sum, taken in split order, to `out` - the result does not depend on which CTA
 // finished first, so a run is bitwise reproducible. out: `rows` x `cols` valid elements, row stride p.ldo; ws holds
 // splits x ceil4(rows * ldo) floats.
 // zcount: grid z extent (splits, or taps x splits for the convolution weight gradient).
@@ -939,9 +944,13 @@ void flpr_gemm_set_debug(int flags) { g_debug = flags; }
 void flpr_gemm_set_generic_epilogue(int on) { g_generic_epi = on; }
 
 // D = alpha * op(A) * op(B)^T.  a_mode/b_mode: 0 = [rows,K] (ld = row stride), 1 = [K,rows] (ld = K-row stride).
-// split_k > 1: fp32 `out` is accumulated into (out += D), deterministically, through `split_ws` (see dispatch_split).
-// col_part (optional, fp32 [ceil(M/128)*4][2][N]): per-32-row partial column sums / sums of squares of the fp32
-// result (fused batch-norm statistics); requires split_k <= 1 and no transposed output.
+// `out` is overwritten with D (after the epilogue) for every split factor.
+// split_k > 1: fp32 output only, summed deterministically through `split_ws` (see dispatch_split). Every split runs
+// the epilogue on its partial product, so bias_n / bias_m / residual / ReLU are refused with split-K; alpha is linear
+// and stays allowed.
+// col_part (optional, fp32 [ceil(M/128)*4][2][N]): per-32-row partial column sums / sums of squares of the stored
+// output (bf16-rounded when the output is bf16; rows >= M count as 0) - the fused batch-norm statistics of
+// alpha * A@B^T. Requires split_k <= 1, no transposed output and no bias / residual / ReLU.
 int flpr_gemm_bf16(const void* A, const void* B, void* out, int M, int N, int K, long long lda, long long ldb,
                    long long ldo, int a_mode, int b_mode, int out_bf16, int trans_out, float alpha,
                    const float* bias_n, const float* bias_m, int relu, const void* residual, int split_k, int bn_req,
@@ -964,6 +973,9 @@ int flpr_gemm_bf16(const void* A, const void* B, void* out, int M, int N, int K,
   p.out = out; p.ldo = ldo; p.out_bf16 = out_bf16; p.trans_out = trans_out;
   if (splits > 1 && out_bf16) return set_err("split-K requires fp32 output", -6);
   if (col_part != nullptr && (splits > 1 || trans_out)) return set_err("col_part needs split_k=1, no transpose", -12);
+  const bool epi = bias_n != nullptr || bias_m != nullptr || relu || residual != nullptr;
+  if (split_k > 1 && epi) return set_err("split-K takes no bias / residual / ReLU (it would apply per split)", -15);
+  if (col_part != nullptr && epi) return set_err("col_part takes no bias / residual / ReLU", -16);
   p.col_part = col_part;
   p.alpha = alpha; p.bias_n = bias_n; p.bias_m = bias_m; p.relu = relu;
   p.residual = reinterpret_cast<const __nv_bfloat16*>(residual);
@@ -1017,6 +1029,8 @@ int flpr_conv_nhwc_bf16(const void* X, const void* Wt, void* out, int NIMG, int 
   bind_device_of(X);
   if (C % 64) return set_err("conv: C must be a multiple of 64", -7);
   if (stride != 1 && stride != 2) return set_err("conv: stride must be 1 or 2", -13);
+  if (col_part != nullptr && (bias_n != nullptr || relu || residual != nullptr))
+    return set_err("conv: col_part takes no bias / residual / ReLU", -16);
   const int Ho = (H + 2 * pad_h - KH) / stride + 1;
   const int Wo = (W + 2 * pad_w - KW) / stride + 1;
   int TH, NB, tiles_per_img, rc;
@@ -1085,10 +1099,10 @@ int flpr_conv_dgrad_nhwc_bf16(const void* dY, const void* Wt, void* out, int NIM
   return dispatch_bn(BN, OP_CONV, OP_TAPFLIP, ta, tb, p, 1, stream, pair_ok(M));
 }
 
-// Weight gradient of a stride-1 convolution: out[Cout, KH*KW*C] (fp32, tap-major then C) +=
+// Weight gradient of a stride-1 convolution: out[Cout, KH*KW*C] (fp32, tap-major then C) =
 //   sum over pixels dY[p, cout] * Xshift_tap[p, c].  One launch covers every tap (grid.z = taps * split_k).
-// dY: [NIMG*H*W, Cout] bf16, X: [NIMG,H,W,C] bf16. split_k > 1: `out` is accumulated into (out += dW) through
-// `split_ws` (splits x ceil4(Cout * KH*KW*C) floats), deterministically (see dispatch_split).
+// dY: [NIMG*H*W, Cout] bf16, X: [NIMG,H,W,C] bf16. `out` is overwritten for every split factor; split_k > 1 sums the
+// splits through `split_ws` (splits x ceil4(Cout * KH*KW*C) floats), deterministically (see dispatch_split).
 int flpr_conv_wgrad_nhwc_bf16(const void* X, const void* dY, float* out, int NIMG, int H, int W, int C, int Cout,
                               int KH, int KW, int pad_h, int pad_w, int split_k, int bn_req, float* split_ws,
                               cudaStream_t stream) {

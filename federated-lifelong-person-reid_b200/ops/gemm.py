@@ -37,8 +37,20 @@ def _split_workspace(split: int, rows: int, ld: int, device) -> Optional[torch.T
     return torch.empty(split * ((rows * ld + 3) // 4 * 4), dtype=torch.float32, device=device)
 
 
+def _check_epilogue(split_k: int, col_part, bias, bias_m, residual, relu: bool) -> None:
+    """Option combinations the kernel cannot compute as one result; refused alike on both devices. A split-K GEMM
+    would run the epilogue once per split (bias added ``split_k`` times, ReLU of each partial), and ``col_part`` holds
+    the statistics of the stored ``alpha * A@B^T``, which has no bias / residual / ReLU."""
+    epi = bias is not None or bias_m is not None or residual is not None or relu
+    if split_k > 1 and epi:
+        raise ValueError("split_k > 1 takes no bias / residual / ReLU epilogue")
+    if col_part is not None and epi:
+        raise ValueError("col_part takes no bias / residual / ReLU epilogue")
+
+
 def _col_part_reference(d: torch.Tensor, col_part: torch.Tensor) -> None:
-    """CPU reference of the fused statistics: 32-row partial sums of ``d`` and ``d*d``."""
+    """CPU reference of the fused statistics: 32-row partial sums of ``d`` and ``d*d`` (``d`` as stored, i.e.
+    already rounded to the output dtype)."""
     m, n = d.shape
     rows = col_part.shape[0]
     pad = rows * 32 - m
@@ -56,21 +68,24 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_kmajor: bool = True, b_kmajor: b
     """``D[M,N] = alpha * A @ B^T`` with bf16 operands and fp32 accumulation.
 
     ``a`` is ``[M,K]`` (``a_kmajor``) or ``[K,M]``; ``b`` is ``[N,K]`` (``b_kmajor``) or ``[K,N]``.
-    Returns ``[M,N]`` (``[N,M]`` when ``trans_out``). ``split_k > 1`` accumulates into a zeroed fp32 output (the
-    splits are summed in a fixed order, so the result is reproducible).
+    Returns ``[M,N]`` (``[N,M]`` when ``trans_out``). ``out`` (optional) is overwritten, whatever ``split_k``.
+    ``split_k > 1`` needs an fp32 output and no bias / residual / ReLU (the splits are summed in a fixed order, so the
+    result is reproducible).
     ``col_part`` (fp32 ``[ceil(M/128)*4, 2, N]``, see :func:`col_part_buffer`) receives per-32-row partial column
-    sums / sums of squares of the fp32 result: the batch-norm statistics pass over the output is fused away.
+    sums / sums of squares of the stored ``alpha * A@B^T`` (rows past ``M`` count as 0): the batch-norm statistics
+    pass over the output is fused away. It takes no bias / residual / ReLU.
     """
     M, K = (a.shape if a_kmajor else (a.shape[1], a.shape[0]))
     N, Kb = (b.shape if b_kmajor else (b.shape[1], b.shape[0]))
     assert K == Kb, f"reduction dims differ: {K} vs {Kb}"
+    _check_epilogue(split_k, col_part, bias_n, bias_m, residual, relu)
     if not a.is_cuda:
         A = a.float() if a_kmajor else a.float().t()
         B = b.float() if b_kmajor else b.float().t()
         A, B = A.to(torch.bfloat16).float(), B.to(torch.bfloat16).float()
         d = alpha * (A @ B.t())
         if col_part is not None:
-            _col_part_reference(d, col_part)
+            _col_part_reference(d.to(out_dtype), col_part)
         if bias_n is not None:
             d = d + bias_n.float()[None, :]
         if bias_m is not None:
@@ -93,10 +108,7 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_kmajor: bool = True, b_kmajor: b
     lda, ldb = a.stride(0), b.stride(0)
     oshape = (N, M) if trans_out else (M, N)
     if out is None:
-        if split_k > 1:
-            out = torch.zeros(oshape, dtype=torch.float32, device=a.device)
-        else:
-            out = torch.empty(oshape, dtype=out_dtype, device=a.device)
+        out = torch.empty(oshape, dtype=torch.float32 if split_k > 1 else out_dtype, device=a.device)
     assert out.stride(-1) == 1
     if split_k > 1:
         assert out.dtype == torch.float32
@@ -120,18 +132,20 @@ def conv_nhwc(x: torch.Tensor, w: torch.Tensor, *, padding: int = 1, out_dtype: 
     """Convolution (stride 1 or 2) as an implicit GEMM. ``x``: ``[N,H,W,C]`` bf16, ``w``: ``[Cout,KH,KW,C]``.
 
     Returns ``[N,Ho,Wo,Cout]``. Zero padding is produced by TMA out-of-bounds fill; a stride-2 convolution walks
-    the input with TMA element strides (same kernel, same pipeline).
+    the input with TMA element strides (same kernel, same pipeline). ``col_part``: see :func:`gemm` (no bias /
+    residual / ReLU with it).
     """
     n, h, wd, c = x.shape
     cout, kh, kw, c2 = w.shape
     assert c == c2
     ho, wo = (h + 2 * padding - kh) // stride + 1, (wd + 2 * padding - kw) // stride + 1
+    _check_epilogue(1, col_part, bias, None, residual, relu)
     if not x.is_cuda:
         xx = x.to(torch.bfloat16).float().permute(0, 3, 1, 2)
         ww = w.to(torch.bfloat16).float().permute(0, 3, 1, 2)
         y = alpha * F.conv2d(xx, ww, padding=padding, stride=stride)
         if col_part is not None:
-            _col_part_reference(y.permute(0, 2, 3, 1).reshape(-1, cout), col_part)
+            _col_part_reference(y.permute(0, 2, 3, 1).reshape(-1, cout).to(out_dtype), col_part)
         if bias is not None:
             y = y + bias.float()[None, :, None, None]
         y = y.permute(0, 2, 3, 1)
@@ -243,8 +257,8 @@ class _LinearFn(torch.autograd.Function):
 def linear(x: torch.Tensor, w_master: torch.Tensor, w_bf16: Optional[torch.Tensor] = None,
            grad_out: Optional[torch.Tensor] = None, want_stats: bool = False, bias: Optional[torch.Tensor] = None):
     """Linear / 1x1-conv on flattened NHWC activations. ``w_master`` fp32 ``[out,in]`` receives the gradient
-    (directly in ``grad_out`` when given - it must be zero on entry). ``want_stats`` additionally returns the fused
-    batch-norm column partials of the output (``(y, part)``)."""
+    (directly in ``grad_out`` when given - it is overwritten, not accumulated into). ``want_stats`` additionally
+    returns the fused batch-norm column partials of the output (``(y, part)``)."""
     if x.is_cuda and (w_master.shape[0] % 8 or w_master.shape[1] % 8 or x.shape[-1] % 8) and not want_stats:
         # TMA needs 16-byte row strides in every operand mode of forward / dgrad / wgrad; a head that is not a
         # multiple of 8 wide (iCaRL grows its classifier by ``n_classes`` at a time, methods/icarl.py) is a tiny GEMM:
@@ -296,7 +310,8 @@ class _Conv3x3Fn(torch.autograd.Function):
 
 def conv3x3_wgrad(x: torch.Tensor, dy: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """dW[Cout,3,3,Cin] (fp32) = sum over pixels of dy (x) shifted x. ONE launch: grid.z enumerates the 9 filter
-    taps (x split-K); the shifted / zero-padded view of ``x`` is produced by 4-D TMA boxes, nothing is copied."""
+    taps (x split-K); the shifted / zero-padded view of ``x`` is produced by 4-D TMA boxes, nothing is copied.
+    ``out`` (optional) is overwritten, whatever split factor the shape gets."""
     n, h, w, cin = x.shape
     cout = dy.shape[-1]
     if not x.is_cuda:
@@ -305,7 +320,7 @@ def conv3x3_wgrad(x: torch.Tensor, dy: torch.Tensor, out: Optional[torch.Tensor]
         g = torch.nn.grad.conv2d_weight(xx, (cout, cin, 3, 3), dd, padding=1)
         g = g.permute(0, 2, 3, 1).contiguous()
         if out is not None:
-            out.add_(g)
+            out.copy_(g)
             return out
         return g
     lib = native.load()
@@ -479,9 +494,11 @@ def stem_conv(x: torch.Tensor, w4: torch.Tensor, bias: Optional[torch.Tensor], r
               col_part: Optional[torch.Tensor] = None) -> torch.Tensor:
     """ResNet stem (7x7 / 2 / pad 3 convolution + folded-BN bias + ReLU) on the implicit-GEMM kernel.
     ``x``: ``[B,H,W,3]`` bf16 NHWC, ``w4``: :func:`stem_weight_s2d` of the (folded) weight. Returns ``[B,H/2,W/2,Cout]``.
-    ``col_part``: fused batch-norm statistics of the output (train-mode BN after an un-folded stem)."""
+    ``col_part``: fused batch-norm statistics of the output (train-mode BN after an un-folded stem); it needs
+    ``bias=None`` and ``relu=False``."""
     b, h, w, _ = x.shape
     cout = w4.shape[0]
+    _check_epilogue(1, col_part, bias, None, None, relu)
     y2 = s2d_pad(x)                                            # [B, H2, W2, 16]
     h2, w2 = h // 2 + 3, w // 2 + 3
     ho, wo = h // 2, w // 2
