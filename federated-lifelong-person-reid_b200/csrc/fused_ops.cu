@@ -244,6 +244,94 @@ __global__ void __launch_bounds__(256) compose_kernel(const float* G, const floa
   }
 }
 
+// ----------------------------------------------------------------------------- server optimizer
+// One step of the server optimizer of adaptive federated optimization (Reddi et al., ICLR 2021, Algorithm 2, without
+// bias correction; FedAvgM, Hsu et al. 2019). x: the server replica's upload prefix, mean: the aggregated uploads.
+// The pseudo-gradient d = mean - x lives in registers only; m, v are fp32.
+//   SOPT_SGD      m = momentum*m + d                                      x += lr*m
+//   SOPT_ADAGRAD  m = b1*m + (1-b1)*d   v = v + d^2                       x += lr*m / (sqrt(v) + tau)
+//   SOPT_ADAM     m = b1*m + (1-b1)*d   v = b2*v + (1-b2)*d^2             x += lr*m / (sqrt(v) + tau)
+//   SOPT_YOGI     m = b1*m + (1-b1)*d   v = v - (1-b2)*d^2*sign(v - d^2)  x += lr*m / (sqrt(v) + tau)
+// The bf16 compute copy of x (nullable) is written in the same pass. This is not fused_opt_kernel: that one is the
+// client hot path (gradient buffer, Adam bias correction, penalties), and sharing it would make it branch on its caller.
+enum { SOPT_SGD = 0, SOPT_ADAGRAD = 1, SOPT_ADAM = 2, SOPT_YOGI = 3 };
+
+struct ServerOptArgs {
+  float* x;
+  const float* mean;
+  float* m;
+  float* v;                  // unused by SOPT_SGD
+  __nv_bfloat16* x_bf16;     // nullable
+  size_t n;
+  float lr, momentum, beta1, beta2, tau;
+};
+
+template <int RULE>
+__device__ __forceinline__ void server_opt_elem(const ServerOptArgs& a, float& x, const float mean, float& m,
+                                                float& v) {
+  const float d = mean - x;
+  if (RULE == SOPT_SGD) {
+    m = a.momentum * m + d;
+    x = x + a.lr * m;
+    return;
+  }
+  m = a.beta1 * m + (1.f - a.beta1) * d;
+  const float d2 = d * d;
+  if (RULE == SOPT_ADAGRAD) {
+    v = v + d2;
+  } else if (RULE == SOPT_ADAM) {
+    v = a.beta2 * v + (1.f - a.beta2) * d2;
+  } else {
+    const float s = v - d2;
+    const float sgn = (s > 0.f) ? 1.f : ((s < 0.f) ? -1.f : 0.f);
+    v = v - (1.f - a.beta2) * d2 * sgn;
+  }
+  x = x + a.lr * m / (sqrtf(v) + a.tau);
+}
+
+// vec: every operand is 16-byte aligned (x_bf16: 8-byte) - float4 accesses over n / 4 quads, then a scalar tail;
+// otherwise scalar accesses throughout.
+template <int RULE>
+__global__ void __launch_bounds__(256) server_opt_kernel(const ServerOptArgs a, const int vec) {
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  const size_t tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  size_t head = 0;
+  if (vec) {
+    const size_t n4 = a.n >> 2;
+    for (size_t i = tid; i < n4; i += stride) {
+      float4 x4 = reinterpret_cast<const float4*>(a.x)[i];
+      const float4 u4 = reinterpret_cast<const float4*>(a.mean)[i];
+      float4 m4 = reinterpret_cast<const float4*>(a.m)[i];
+      float4 v4 = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (RULE != SOPT_SGD) v4 = reinterpret_cast<const float4*>(a.v)[i];
+      server_opt_elem<RULE>(a, x4.x, u4.x, m4.x, v4.x);
+      server_opt_elem<RULE>(a, x4.y, u4.y, m4.y, v4.y);
+      server_opt_elem<RULE>(a, x4.z, u4.z, m4.z, v4.z);
+      server_opt_elem<RULE>(a, x4.w, u4.w, m4.w, v4.w);
+      reinterpret_cast<float4*>(a.x)[i] = x4;
+      reinterpret_cast<float4*>(a.m)[i] = m4;
+      if (RULE != SOPT_SGD) reinterpret_cast<float4*>(a.v)[i] = v4;
+      if (a.x_bf16) {
+        __nv_bfloat162 lo = __floats2bfloat162_rn(x4.x, x4.y), hi = __floats2bfloat162_rn(x4.z, x4.w);
+        uint2 u;
+        u.x = *reinterpret_cast<uint32_t*>(&lo);
+        u.y = *reinterpret_cast<uint32_t*>(&hi);
+        reinterpret_cast<uint2*>(a.x_bf16)[i] = u;
+      }
+    }
+    head = n4 << 2;
+  }
+  for (size_t i = head + tid; i < a.n; i += stride) {
+    float x = a.x[i], m = a.m[i], v = 0.f;
+    if (RULE != SOPT_SGD) v = a.v[i];
+    server_opt_elem<RULE>(a, x, a.mean[i], m, v);
+    a.x[i] = x;
+    a.m[i] = m;
+    if (RULE != SOPT_SGD) a.v[i] = v;
+    if (a.x_bf16) a.x_bf16[i] = __float2bfloat16_rn(x);
+  }
+}
+
 // ----------------------------------------------------------------------------- label-smoothing CE
 // One block per sample. logits: [B, C] (bf16 or fp32, row stride ld). dlogits same layout (bf16 or fp32).
 // row_part[2 row] = loss_row / B, row_part[2 row + 1] = (argmax == target); ce_stats_kernel folds them into stats.
@@ -1277,6 +1365,29 @@ int flpr_compose(const float* G, const float* A, float a, float* theta, void* th
   bind_device_of(G);
   if (n % 4) return -2;
   compose_kernel<<<grid_for(n / 4, 256), 256, 0, st>>>(G, A, a, theta, reinterpret_cast<__nv_bfloat16*>(theta_bf16), n);
+  return (int)cudaGetLastError();
+}
+
+// rule: SOPT_SGD 0, SOPT_ADAGRAD 1, SOPT_ADAM 2, SOPT_YOGI 3 (see server_opt_kernel). x, mean, m are required, v for
+// every rule but SOPT_SGD; x_bf16 is nullable. Any length and alignment. -2: unknown rule, -3: a required pointer is null.
+int flpr_server_opt(int rule, float* x, const float* mean, float* m, float* v, void* x_bf16, size_t n, float lr,
+                    float momentum, float beta1, float beta2, float tau, cudaStream_t st) {
+  if (rule < SOPT_SGD || rule > SOPT_YOGI) return -2;
+  if (x == nullptr || mean == nullptr || m == nullptr || (rule != SOPT_SGD && v == nullptr)) return -3;
+  if (n == 0) return 0;
+  bind_device_of(x);
+  ServerOptArgs a;
+  a.x = x; a.mean = mean; a.m = m; a.v = v; a.x_bf16 = reinterpret_cast<__nv_bfloat16*>(x_bf16); a.n = n;
+  a.lr = lr; a.momentum = momentum; a.beta1 = beta1; a.beta2 = beta2; a.tau = tau;
+  const auto al = [](const void* p, uintptr_t b) { return (reinterpret_cast<uintptr_t>(p) & (b - 1)) == 0; };
+  const int vec = al(x, 16) && al(mean, 16) && al(m, 16) && (rule == SOPT_SGD || al(v, 16)) && al(x_bf16, 8);
+  const int grid = grid_for(vec ? (n + 3) / 4 : n, 256);
+  switch (rule) {
+    case SOPT_SGD: server_opt_kernel<SOPT_SGD><<<grid, 256, 0, st>>>(a, vec); break;
+    case SOPT_ADAGRAD: server_opt_kernel<SOPT_ADAGRAD><<<grid, 256, 0, st>>>(a, vec); break;
+    case SOPT_ADAM: server_opt_kernel<SOPT_ADAM><<<grid, 256, 0, st>>>(a, vec); break;
+    default: server_opt_kernel<SOPT_YOGI><<<grid, 256, 0, st>>>(a, vec); break;
+  }
   return (int)cudaGetLastError();
 }
 

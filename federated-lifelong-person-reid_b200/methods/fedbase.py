@@ -18,6 +18,7 @@ from typing import Any, Dict, List, Optional
 
 import torch
 
+from ..ops import fused as fops
 from ..ops import layer as lops
 from ..runtime.modules import ClientModule, ModelModule, ServerModule
 
@@ -126,17 +127,65 @@ class FedClient(ClientModule):
         self.train_cnt += output["data_count"]              # methods/fedavg.py:298
 
 
+_SERVER_OPT_KEYS = {"sgd": {"lr": None, "momentum": 0.0}}
+_SERVER_OPT_KEYS.update({name: {"lr": None, "beta1": 0.9, "beta2": 0.99, "tau": 1e-3}
+                         for name in ("adagrad", "adam", "yogi")})
+
+
+def parse_server_opt(cfg: Optional[Dict]) -> Optional[Dict[str, Any]]:
+    """Validate the ``server: server_opt:`` block, e.g. ``{name: adam, lr: 0.01, beta1: 0.9, beta2: 0.99, tau: 0.001}``,
+    and return it with the defaults filled in (``None``: no block, plain FedAvg replacement of the replica).
+    ``sgd`` takes ``lr`` and ``momentum``; ``adagrad`` / ``adam`` / ``yogi`` take ``lr``, ``beta1``, ``beta2`` (unused by
+    ``adagrad``) and ``tau``. Raises ``ValueError`` on an unknown name or key, a missing or non-positive ``lr``, a
+    ``momentum`` / ``beta1`` / ``beta2`` outside ``[0, 1)`` or a non-positive ``tau``."""
+    if cfg is None:
+        return None
+    if not isinstance(cfg, dict):
+        raise ValueError(f"server_opt must be a mapping, got {cfg!r}")
+    name = cfg.get("name")
+    if name not in _SERVER_OPT_KEYS:
+        raise ValueError(f"server_opt: unknown name {name!r} (one of {sorted(_SERVER_OPT_KEYS)})")
+    allowed = _SERVER_OPT_KEYS[name]
+    unknown = sorted(set(cfg) - set(allowed) - {"name"})
+    if unknown:
+        raise ValueError(f"server_opt: unknown key(s) {unknown} for {name!r} (allowed: {sorted(allowed)})")
+    if "lr" not in cfg:
+        raise ValueError("server_opt: lr is required")
+    out: Dict[str, Any] = {"name": name}
+    for key, default in allowed.items():
+        try:
+            out[key] = float(cfg.get(key, default))
+        except (TypeError, ValueError):
+            raise ValueError(f"server_opt: {key} must be a number, got {cfg.get(key)!r}") from None
+    if not out["lr"] > 0:
+        raise ValueError(f"server_opt: lr must be > 0, got {out['lr']}")
+    for key in ("momentum", "beta1", "beta2"):
+        if key in out and not 0 <= out[key] < 1:
+            raise ValueError(f"server_opt: {key} must be in [0, 1), got {out[key]}")
+    if "tau" in out and not out["tau"] > 0:
+        raise ValueError(f"server_opt: tau must be > 0, got {out['tau']}")
+    return out
+
+
 class FedServer(ServerModule):
-    """Server role of the FedAvg-family exchange (replicated on every rank)."""
+    """Server role of the FedAvg-family exchange (replicated on every rank).
+
+    ``server_opt`` (optional, :func:`parse_server_opt`): instead of overwriting the replica with the aggregated mean,
+    ``calculate()`` takes one server-optimizer step toward it (FedAvgM / FedAdagrad / FedAdam / FedYogi,
+    ``ops.fused.server_opt_step``). ``glob`` is bitwise identical on every rank, so the replicated step keeps the replicas
+    (and their moments ``m`` / ``v``) identical without any extra communication."""
 
     upload_key = "incremental_model_params"
     integrated_key = "integrated_model_params"
     payload_prefix = "net."
 
-    def __init__(self, server_name, model, operator, ckpt_root, **kwargs):
+    def __init__(self, server_name, model, operator, ckpt_root, server_opt: Optional[Dict] = None, **kwargs):
         super().__init__(server_name, model, operator, ckpt_root, **kwargs)
         self.client_ids: Dict[str, int] = {}
         self.uploaded: List[int] = []                       # client ids with a valid upload slot (insertion order)
+        self.server_opt = parse_server_opt(server_opt)
+        self.opt_m: Optional[torch.Tensor] = None           # server-optimizer moments, fp32, allocated on first use
+        self.opt_v: Optional[torch.Tensor] = None
 
     def bind_client(self, client_name: str, client_id: int) -> None:
         self.client_ids[client_name] = client_id
@@ -162,10 +211,36 @@ class FedServer(ServerModule):
 
     def calculate(self) -> Any:
         glob = self.aggregate()
-        if glob is not None:
-            a = self.model.arena
+        if glob is None:
+            return
+        a = self.model.arena
+        if self.server_opt is None:
             a.master[:glob.numel()].copy_(glob)
             a.refresh_shadow()
+            return
+        n, o = glob.numel(), self.server_opt
+        if self.opt_m is None:
+            self.opt_m = torch.zeros(n, dtype=torch.float32, device=a.device)
+            if o["name"] != "sgd":
+                self.opt_v = torch.zeros(n, dtype=torch.float32, device=a.device)
+        # (the arena tail beyond the upload prefix never changes here, so its bf16 copy stays current)
+        fops.server_opt_step(o["name"], a.master[:n], glob, self.opt_m, self.opt_v, lr=o["lr"],
+                             momentum=o.get("momentum", 0.0), beta1=o.get("beta1", 0.9), beta2=o.get("beta2", 0.99),
+                             tau=o.get("tau", 1e-3), x_bf16=None if a.shadow is None else a.shadow[:n])
+
+    def resume_extra(self) -> Dict[str, Any]:
+        """The server-optimizer moments (replicated like the replica itself); ``{}`` without ``server_opt``."""
+        if self.server_opt is None:
+            return {}
+        return {"server_opt_m": self.opt_m, "server_opt_v": self.opt_v}
+
+    def load_resume_extra(self, extra: Dict[str, Any]) -> None:
+        if self.server_opt is None:
+            return
+        dev = self.model.arena.device
+        m, v = extra.get("server_opt_m"), extra.get("server_opt_v")
+        self.opt_m = None if m is None else m.to(dev, torch.float32).clone()
+        self.opt_v = None if v is None else v.to(dev, torch.float32).clone()
 
     def _named_global(self) -> Dict[str, torch.Tensor]:
         a = self.model.arena

@@ -90,6 +90,56 @@ def fused_optimizer_step(kind: str, p: torch.Tensor, g: torch.Tensor, m: Optiona
     native.count_launch()
 
 
+SERVER_OPT_RULES = ("sgd", "adagrad", "adam", "yogi")           # index = the ``rule`` code of ``flpr_server_opt``
+
+
+def _f32(s: float) -> float:
+    return float(torch.tensor(s, dtype=torch.float32))
+
+
+def server_opt_step(rule: str, x: torch.Tensor, mean: torch.Tensor, m: torch.Tensor, v: Optional[torch.Tensor], *,
+                    lr: float, momentum: float = 0.0, beta1: float = 0.9, beta2: float = 0.99, tau: float = 1e-3,
+                    x_bf16: Optional[torch.Tensor] = None) -> None:
+    """One in-place server-optimizer step (Reddi et al., "Adaptive Federated Optimization", Algorithm 2, no bias
+    correction; ``sgd`` is FedAvgM, Hsu et al. 2019) over flat fp32 ``x`` (the server replica) toward ``mean`` (the
+    aggregated uploads). With ``d = mean - x``:
+
+    * ``sgd``:     ``m = momentum*m + d``;                                 ``x = x + lr*m``
+    * ``adagrad``: ``m = beta1*m + (1-beta1)*d``; ``v = v + d^2``;          ``x = x + lr*m / (sqrt(v) + tau)``
+    * ``adam``:    ``m = beta1*m + (1-beta1)*d``; ``v = beta2*v + (1-beta2)*d^2``;             (same ``x`` update)
+    * ``yogi``:    ``m = beta1*m + (1-beta1)*d``; ``v = v - (1-beta2)*d^2*sign(v - d^2)``;     (same ``x`` update)
+
+    ``m`` / ``v`` are fp32 state of ``x``'s size (``v`` unused by ``sgd``, may be ``None`` there); ``x_bf16`` (optional)
+    receives the bf16 copy of the new ``x``. CUDA: one pass of ``server_opt_kernel``; CPU: the same formulas in fp32
+    tensor ops, in the same order."""
+    code = SERVER_OPT_RULES.index(rule)
+    if not _native(x, "flpr_server_opt"):
+        b1, b2 = _f32(beta1), _f32(beta2)                   # 1 - b then rounds like the kernel's fp32 ``1.f - b``
+        with torch.no_grad():
+            d = mean - x
+            if rule == "sgd":
+                m.mul_(momentum).add_(d)
+                x.add_(lr * m)
+            else:
+                m.mul_(b1).add_((1 - b1) * d)
+                d2 = d * d
+                if rule == "adagrad":
+                    v.add_(d2)
+                elif rule == "adam":
+                    v.mul_(b2).add_((1 - b2) * d2)
+                else:
+                    v.sub_((1 - b2) * d2 * torch.sign(v - d2))
+                x.add_(lr * m / (v.sqrt() + tau))
+            if x_bf16 is not None:
+                x_bf16.copy_(x)
+        return
+    lib = _lib()
+    rc = lib.flpr_server_opt(code, native.ptr(x), native.ptr(mean), native.ptr(m), native.ptr(v), native.ptr(x_bf16),
+                             x.numel(), lr, momentum, beta1, beta2, tau, _stream(x.device))
+    native.check(rc, "flpr_server_opt")
+    native.count_launch()
+
+
 def importance_accumulate(Fbuf: torch.Tensor, g: torch.Tensor, scale: float, mode: str = "fisher") -> None:
     """``F += scale * g**2`` (fisher) or ``F += scale * |g|`` (mas)."""
     if not _native(Fbuf):

@@ -60,6 +60,7 @@ def _signatures() -> dict:
         "flpr_importance_accum": [P, P, Z, F, I, P],
         "flpr_cast_bf16": [P, P, Z, P],
         "flpr_compose": [P, P, F, P, P, Z, P],
+        "flpr_server_opt": [I, P, P, P, P, P, Z, F, F, F, F, F, P],
         "flpr_ce_label_smooth": [P, P, P, P, P, I, I, L, F, F, I, I, P],
         "flpr_bn_fwd": [P, P, P, P, P, P, P, P, P, P, P, P, I, I, F, F, I, P, I, P],
         "flpr_affine_act": [P, P, P, P, P, I, I, I, P],
