@@ -5,7 +5,8 @@
 //                     2*lam*(Q*p - R)  [EWC ewc.py:80-85, MAS mas.py:78-83, FedProx fedprox.py:52-57,
 //                     FedCurv fedcurv.py:79-86 all reduce to this form], (b) FedSTIL's L1 sparseness gradient
 //                     lam1*sign(theta - G) and adaptive-weight decay (fedstil.py:639-644), (c) the bf16 compute
-//                     copy of the updated weights, (d) the penalty / L1 *values* for loss reporting.
+//                     copy of the updated weights, (d) the penalty / L1 *values* for loss reporting, (e) with the SI
+//                     flag, the Synaptic Intelligence path integral omega += -g * (p_new - p_old).
 //   importance_accum  Fisher (g^2) / MAS (|g|) accumulation (ewc.py:56-78, mas.py:55-76, fedcurv.py:56-77).
 //   ce_label_smooth   fused log-softmax + label-smoothing CE + gradient + top-1 hit count
 //                     (criterions/cross_entropy.py:35-40 and the per-step accuracy at baseline.py:47).
@@ -59,9 +60,13 @@ struct OptArgs {
   float* anchor;
   float* am;
   float* av;
+  // Synaptic Intelligence path integral (Zenke et al. 2017, Eq. 4), read and written by the SI instantiation only:
+  // omega += -g * (p_new - p_old) per element, with g the loss gradient as passed in (before the L1, penalty and
+  // weight-decay terms). Last field, so the offsets of the others are those of the non-SI kernels.
+  float* omega;
 };
 
-template <bool ADAM>
+template <bool ADAM, bool SI>
 __global__ void __launch_bounds__(256) fused_opt_kernel(const OptArgs a) {
   __shared__ float sh[8];
   float pen = 0.f, l1 = 0.f;
@@ -83,6 +88,9 @@ __global__ void __launch_bounds__(256) fused_opt_kernel(const OptArgs a) {
     if (a.Q) q4 = reinterpret_cast<const float4*>(a.Q)[i];
     if (a.R) r4 = reinterpret_cast<const float4*>(a.R)[i];
     if (a.G) G4 = reinterpret_cast<const float4*>(a.G)[i];
+    float4 w4 = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (SI) w4 = reinterpret_cast<const float4*>(a.omega)[i];
+    float* ww = reinterpret_cast<float*>(&w4);
     float4 c4 = G4, cm4 = make_float4(0.f, 0.f, 0.f, 0.f), cv4 = cm4;
     if (a.anchor) {
       c4 = reinterpret_cast<const float4*>(a.anchor)[i];
@@ -156,8 +164,10 @@ __global__ void __launch_bounds__(256) fused_opt_kernel(const OptArgs a) {
         np = p - lr * d;
       }
       pp[t] = np;
+      if (SI) ww[t] = fmaf(-gg[t], np - p, ww[t]);
     }
     reinterpret_cast<float4*>(a.p)[i] = p4;
+    if (SI) reinterpret_cast<float4*>(a.omega)[i] = w4;
     if (ADAM || a.momentum != 0.f) reinterpret_cast<float4*>(a.m)[i] = m4;
     if (ADAM) reinterpret_cast<float4*>(a.v)[i] = v4;
     if (a.anchor) {
@@ -1320,11 +1330,12 @@ using namespace flpr;
 extern "C" {
 
 // stats_part (required with stats): 2 x 1056 floats of scratch (2 per block, at most 132 * 8 blocks).
+// omega (nullable): Synaptic Intelligence path integral, accumulated by the SI instantiation of the kernel.
 int flpr_fused_opt(int adam, float* p, const float* g, float* m, float* v, const float* Q, const float* R,
                    const float* G, void* p_bf16, float* stats, size_t n, float lr, float beta1, float beta2, float eps,
                    float wd, int step, float lam2, float lam1, float atten, float momentum, int penalty_ones,
                    const float* hyper, float* anchor, float* anchor_m, float* anchor_v, float* stats_part,
-                   cudaStream_t st) {
+                   float* omega, cudaStream_t st) {
   bind_device_of(p);
   if (n % 4) return -2;
   OptArgs a;
@@ -1335,14 +1346,20 @@ int flpr_fused_opt(int adam, float* p, const float* g, float* m, float* v, const
   a.bc2_sqrt = sqrtf(1.f - powf(beta2, (float)step));
   a.lam2 = lam2; a.lam1 = lam1; a.atten = atten; a.momentum = momentum; a.penalty_ones = penalty_ones;
   a.hyper = hyper;
+  a.omega = omega;
   a.anchor = G != nullptr ? anchor : nullptr; a.am = anchor_m; a.av = anchor_v;
   if (a.anchor != nullptr && ((adam && (anchor_m == nullptr || anchor_v == nullptr)) ||
                               (!adam && momentum != 0.f && anchor_m == nullptr)))
     return -3;
   if (stats != nullptr && stats_part == nullptr) return -4;
   const int grid = grid_for(n / 4, 256);
-  if (adam) fused_opt_kernel<true><<<grid, 256, 0, st>>>(a);
-  else fused_opt_kernel<false><<<grid, 256, 0, st>>>(a);
+  if (omega != nullptr) {
+    if (adam) fused_opt_kernel<true, true><<<grid, 256, 0, st>>>(a);
+    else fused_opt_kernel<false, true><<<grid, 256, 0, st>>>(a);
+  } else {
+    if (adam) fused_opt_kernel<true, false><<<grid, 256, 0, st>>>(a);
+    else fused_opt_kernel<false, false><<<grid, 256, 0, st>>>(a);
+  }
   if (stats != nullptr) opt_stats_kernel<<<1, 32, 0, st>>>(stats_part, stats, grid, R != nullptr, G != nullptr);
   return (int)cudaGetLastError();
 }

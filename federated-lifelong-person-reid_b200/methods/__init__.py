@@ -6,6 +6,7 @@ _NAMES = {
     "baseline": "baseline",
     "ewc": "ewc",
     "mas": "mas",
+    "si": "si",
     "icarl": "icarl",
     "fedavg": "fedavg",
     "fedprox": "fedprox",

@@ -33,7 +33,7 @@ def fused_optimizer_step(kind: str, p: torch.Tensor, g: torch.Tensor, m: Optiona
                          atten: float = 0.0, p_bf16: Optional[torch.Tensor] = None,
                          stats: Optional[torch.Tensor] = None, hyper: Optional[torch.Tensor] = None,
                          anchor: Optional[torch.Tensor] = None, anchor_m: Optional[torch.Tensor] = None,
-                         anchor_v: Optional[torch.Tensor] = None) -> None:
+                         anchor_v: Optional[torch.Tensor] = None, omega: Optional[torch.Tensor] = None) -> None:
     """One in-place optimizer step over a flat fp32 arena.
 
     gradient used:  g + wd * (p - atten*G) + 2*lam2*(Q*p - R) + lam1*sign(p - G)
@@ -43,6 +43,9 @@ def fused_optimizer_step(kind: str, p: torch.Tensor, g: torch.Tensor, m: Optiona
     ``anchor`` (CUDA only; the CPU twin is ``ArenaOptimizer._anchor_step``): FedSTIL's *trained* L1 anchor
     ``theta0 = atten*G + aw0`` replaces ``G`` in the L1 term and is itself stepped in the same pass with gradient
     ``-lam1*sign(p - theta0) + wd*(theta0 - atten*G)`` and its own moments (reference ``fedstil.py:53-76,639-647``).
+
+    ``omega`` (optional): Synaptic Intelligence path integral, ``omega += -g * (p_new - p_old)`` with ``g`` the gradient
+    as passed in (without the penalty, weight-decay and L1 terms) and ``p_new - p_old`` the update this step applied.
     """
     adam = kind == "adam"
     if hyper is not None and not _native(p):
@@ -50,6 +53,7 @@ def fused_optimizer_step(kind: str, p: torch.Tensor, g: torch.Tensor, m: Optiona
     if not _native(p):
         assert anchor is None, "the CPU path of the trained anchor is ArenaOptimizer._anchor_step"
         with torch.no_grad():
+            p_before = None if omega is None else p.clone()
             grad = g.clone()
             base = p
             if G is not None:
@@ -76,6 +80,8 @@ def fused_optimizer_step(kind: str, p: torch.Tensor, g: torch.Tensor, m: Optiona
                     m.mul_(momentum).add_(grad)
                     grad = m
                 p.add_(grad, alpha=-lr)
+            if omega is not None:
+                omega.sub_(g * (p - p_before))
             if p_bf16 is not None:
                 p_bf16.copy_(p)
         return
@@ -85,7 +91,7 @@ def fused_optimizer_step(kind: str, p: torch.Tensor, g: torch.Tensor, m: Optiona
                             beta2, eps, weight_decay, int(step), lam2, lam1, atten, momentum, int(penalty_ones),
                             native.ptr(hyper), native.ptr(anchor if G is not None else None), native.ptr(anchor_m),
                             native.ptr(anchor_v), native.ptr(None if stats is None else _opt_stats_scratch(p.device)),
-                            _stream(p.device))
+                            native.ptr(omega), _stream(p.device))
     native.check(rc, "flpr_fused_opt")
     native.count_launch()
 

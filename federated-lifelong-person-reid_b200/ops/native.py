@@ -56,7 +56,7 @@ def _signatures() -> dict:
         "flpr_comm_curv_moments": [I, I, P, D, I, P, P, P, P, P, Z, I, P],
         "flpr_comm_gather_strided": [I, I, P, D, I, P, P, Z, I, P],
         "flpr_comm_pull_copy": [I, I, P, D, P, P, P, Z, I, P],
-        "flpr_fused_opt": [I, P, P, P, P, P, P, P, P, P, Z, F, F, F, F, F, I, F, F, F, F, I, P, P, P, P, P, P],
+        "flpr_fused_opt": [I, P, P, P, P, P, P, P, P, P, Z, F, F, F, F, F, I, F, F, F, F, I, P, P, P, P, P, P, P],
         "flpr_importance_accum": [P, P, Z, F, I, P],
         "flpr_cast_bf16": [P, P, Z, P],
         "flpr_compose": [P, P, F, P, P, Z, P],

@@ -156,6 +156,9 @@ class ArenaOptimizer:
         self.anchor: Optional[torch.Tensor] = None
         self.anchor_m: Optional[torch.Tensor] = None
         self.anchor_v: Optional[torch.Tensor] = None
+        # Synaptic Intelligence path integral (methods/si.py), accumulated by the step; must stay the same tensor while
+        # a CUDA graph of the step is live
+        self.omega: Optional[torch.Tensor] = None
         # device-resident [lr, step] (CUDA only): a captured CUDA graph of the train step stays valid across steps
         self.hyper: Optional[torch.Tensor] = None
         if arena.device.type == "cuda":
@@ -194,6 +197,8 @@ class ArenaOptimizer:
 
     def step(self) -> None:
         a = self.arena
+        if self.omega is not None and (self.G is not None or self.anchor is not None):
+            raise ValueError("the SI path integral (omega) cannot be combined with FedSTIL's G / trained L1 anchor")
         if self.m is None and (self.kind == "adam" or self.defaults["momentum"] != 0.0):
             self.m = a.new_buffer()
         if self.v is None and self.kind == "adam":
@@ -224,7 +229,8 @@ class ArenaOptimizer:
                 p_bf16=None if a.shadow is None else a.shadow[sl], stats=self.stats, hyper=self.hyper,
                 anchor=self.anchor[sl] if anc else None,
                 anchor_m=self.anchor_m[sl] if anc and self.anchor_m is not None else None,
-                anchor_v=self.anchor_v[sl] if anc and self.anchor_v is not None else None)
+                anchor_v=self.anchor_v[sl] if anc and self.anchor_v is not None else None,
+                omega=None if self.omega is None else self.omega[sl])
 
         lam1, l1_before = self.lam1, None
         if trained_anchor and not fused_anchor:

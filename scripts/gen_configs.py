@@ -2,6 +2,8 @@
 9 backbone experiments, 22 FedSTIL hyper-parameter sweeps - same ``exp_name`` / ``exp_method`` / hyper-parameters, so
 ``python main.py --experiments configs/basis_exp/experiment_fedstil.yaml`` means the same run) and the B200 workloads
 named in BASELINE.json (``configs/b200/``: ResNet-50 / Swin-T, 8 clients x 5 tasks, 256x128, bf16).
+Synaptic Intelligence (``basis_exp/experiment_si.yaml``, ``b200/experiment_si_res50_1.yaml``) is this project's
+addition next to the reference's EWC / MAS experiments.
 
 The experiment definitions are parameter tables below; files are emitted in a compact flow style."""
 import os
@@ -57,6 +59,8 @@ BASIS = {
             "clients": clients()},
     "mas": {"exp_name": "mas", "exp_method": "mas", "model_opts": net(lambda_penalty=0.01), "server": dict(SERVER),
             "clients": clients()},
+    "si": {"exp_name": "si", "exp_method": "si", "model_opts": net(lambda_penalty=0.1, si_xi=1e-3),
+           "server": dict(SERVER), "clients": clients()},
     "icarl": {"exp_name": "icarl", "exp_method": "icarl", "server": dict(SERVER),
               "model_opts": dict(net(k=12000, n_classes=10, examplar_batch_size=64), num_classes=10),
               "clients": clients()},
@@ -128,6 +132,8 @@ B200 = {
                         exp_opts={"comm_rounds": 50, "val_interval": 10, "online_clients": 1}),
     "mas_res50_1": dict(b200("b200-mas-res50", "mas", "resnet50", lambda_penalty=0.01), clients=clients(1, 5),
                         exp_opts={"comm_rounds": 50, "val_interval": 10, "online_clients": 1}),
+    "si_res50_1": dict(b200("b200-si-res50", "si", "resnet50", lambda_penalty=0.1, si_xi=1e-3), clients=clients(1, 5),
+                       exp_opts={"comm_rounds": 50, "val_interval": 10, "online_clients": 1}),
     "icarl_res50_1": dict(b200("b200-icarl-res50", "icarl", "resnet50", k=12000, n_classes=10), clients=clients(1, 5),
                           exp_opts={"comm_rounds": 50, "val_interval": 10, "online_clients": 1}),
 }
