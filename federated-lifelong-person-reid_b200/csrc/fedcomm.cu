@@ -23,6 +23,9 @@
 //                            multimem.ld_reduce adds the partials of all ranks INSIDE THE SWITCH for this rank's slice,
 //                            the kernel scales by 1 / sum k and multimem.st broadcasts the slice to every rank's
 //                            destination: each GPU sends and receives the buffer once, whatever the number of ranks.
+//   fed_reduce_robust C1+C2  Byzantine-robust aggregate: coordinate-wise median or trimmed mean of the K uploads
+//                            (unweighted), same two-shot structure as fed_reduce_bcast; every coordinate's K values are
+//                            sorted in registers by a sorting network.
 //
 // Clients-per-rank is arbitrary (8 clients on 1/2/4/8 GPUs): sources are a table of K pointers, local or peer.
 // Concurrent collectives (aggregation on a communication stream while the next round's mix runs on the compute stream)
@@ -270,6 +273,137 @@ fed_reduce_bcast_nvls_kernel(const CommCtx ctx, const NvlsReduceArgs a) {
   }
   rank_barrier(ctx, e0 + 3);  // every slice has landed everywhere
   block_epoch_end(ctx, e0 + 3);
+}
+
+// ----------------------------------------------------------------------------- C1 + C2 robust (median / trimmed mean)
+// Order of the K values of one coordinate: (value, position in the client list), NaN above +inf, -0.0 == +0.0 (the
+// tie goes to the lower position) - what a stable sort of the K values gives. Each value becomes one 64-bit key that
+// sorts in exactly that order and still holds the value's bits:
+//   high word  order key of the value: NaN -> 0xFFFFFFFF, +-0 -> 0x80000000, x > 0 -> bits | 0x80000000, x < 0 -> ~bits
+//   low word   [31:27] position, [23] sign bit, [22:0] mantissa
+// The exponent is recovered from the high word (negative values: from ~high), so the key decodes to the original bits,
+// signed zeros and NaN payloads included. The padding of a K-bucket (all ones) sorts after every real key.
+constexpr int ROBUST_MEDIAN = 0;
+constexpr int ROBUST_TRIMMED_MEAN = 1;
+
+struct RobustArgs {
+  int K;                              // number of client sources
+  int rule;                           // ROBUST_MEDIAN / ROBUST_TRIMMED_MEAN
+  int b;                              // trimmed mean: sorted positions [b, K - b) are kept
+  const float* src[MAX_CLIENTS];      // upload buffers (local or peer)
+  float* dst[MAX_RANKS];              // destination buffer on every rank (peer-mapped)
+  size_t n4;                          // length in float4
+};
+
+__device__ __forceinline__ uint32_t f32_bits(float x) {
+#ifdef __CUDA_ARCH__
+  return __float_as_uint(x);
+#else
+  uint32_t u;
+  memcpy(&u, &x, 4);
+  return u;
+#endif
+}
+
+__device__ __forceinline__ unsigned long long robust_key(float x, int pos) {
+  const uint32_t u = f32_bits(x);
+  const uint32_t ax = u & 0x7FFFFFFFu;
+  const uint32_t hi = ax > 0x7F800000u ? 0xFFFFFFFFu : (ax == 0u ? 0x80000000u : ((u >> 31) ? ~u : (u | 0x80000000u)));
+  const uint32_t lo = ((uint32_t)pos << 27) | ((u >> 31) << 23) | (u & 0x007FFFFFu);
+  return ((unsigned long long)hi << 32) | lo;
+}
+
+__device__ __forceinline__ float robust_value(unsigned long long key) {
+  const uint32_t hi = (uint32_t)(key >> 32), lo = (uint32_t)key;
+  const uint32_t e = (((hi >> 31) ? hi : ~hi) >> 23) & 0xFFu;
+  return __uint_as_float((((lo >> 23) & 1u) << 31) | (e << 23) | (lo & 0x007FFFFFu));
+}
+
+__device__ __forceinline__ void cmp_swap(unsigned long long& a, unsigned long long& b) {
+  const bool s = a > b;
+  const unsigned long long lo = s ? b : a;
+  b = s ? a : b;
+  a = lo;
+}
+
+// Batcher's odd-even merge sort of P = 2^LOG keys. Stage (p, d) with p = 2^lp, d = 2^(lp - ld) compares x and x + d
+// for every x with (x - d % p) mod 2d < d inside one block of 2p. Every loop has a constant trip count, so full
+// unrolling turns every index into a constant and the keys stay in registers.
+template <int P, int LOG>
+__device__ __forceinline__ void sort_keys(unsigned long long (&k)[P]) {
+#pragma unroll
+  for (int lp = 0; lp < LOG; ++lp)
+#pragma unroll
+    for (int ld = 0; ld < LOG; ++ld)
+#pragma unroll
+      for (int x = 0; x < P; ++x) {
+        const int p = 1 << lp, d = ld <= lp ? 1 << (lp - ld) : 1, r = d % p;
+        if (ld <= lp && x + d < P && x >= r && (x - r) % (2 * d) < d && x / (2 * p) == (x + d) / (2 * p))
+          cmp_swap(k[x], k[x + d]);
+      }
+}
+
+// (0.5 * lo + 0.5 * hi, each product and the sum rounded on its own: no FMA contraction)
+__device__ __forceinline__ float robust_midpoint(float lo, float hi) {
+#ifdef __CUDA_ARCH__
+  return __fadd_rn(__fmul_rn(0.5f, lo), __fmul_rn(0.5f, hi));
+#else
+  return 0.5f * lo + 0.5f * hi;  // (host builds are ISO C++: no contraction)
+#endif
+}
+
+template <int P, int LOG>
+__device__ __forceinline__ void robust_body(const CommCtx& ctx, const RobustArgs& a, size_t e_lo, size_t e_hi) {
+  const int K = a.K;
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  for (size_t e = e_lo + (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < e_hi; e += stride) {
+    unsigned long long k[P];
+#pragma unroll
+    for (int c = 0; c < P; ++c) k[c] = c < K ? robust_key(a.src[c][e], c) : ~0ull;
+    sort_keys<P, LOG>(k);
+    float out;
+    if (a.rule == ROBUST_MEDIAN) {
+      // odd K: position (K-1)/2; even K: midpoint of positions K/2-1 and K/2
+      const int m_lo = (K - 1) >> 1, m_hi = K >> 1;
+      unsigned long long lo = 0ull, hi = 0ull;
+#pragma unroll
+      for (int j = 0; j < P; ++j) {
+        if (j == m_lo) lo = k[j];
+        if (j == m_hi) hi = k[j];
+      }
+      out = (m_lo == m_hi) ? robust_value(lo) : robust_midpoint(robust_value(lo), robust_value(hi));
+    } else {
+      // sum of the kept positions in ascending order; -0.0 is the exact identity of the addition
+      float acc = -0.f;
+#pragma unroll
+      for (int j = 0; j < P; ++j)
+        if (j >= a.b && j < K - a.b) acc += robust_value(k[j]);
+      out = acc / (float)(K - 2 * a.b);
+    }
+#pragma unroll
+    for (int r = 0; r < MAX_RANKS; ++r)
+      if (r < ctx.world) a.dst[r][e] = out;
+  }
+}
+
+__global__ void __launch_bounds__(COMM_THREADS)
+fed_reduce_robust_kernel(const CommCtx ctx, const RobustArgs a) {
+  const uint32_t e0 = block_epoch_begin(ctx);
+  const bool ok = rank_barrier(ctx, e0 + 1);  // all uploads are complete on every rank
+  // two-shot: this rank reduces slice [lo, hi) (in float4 units, as fed_reduce_bcast) and pushes it to every rank
+  const size_t per = (a.n4 + ctx.world - 1) / ctx.world;
+  const size_t lo = per * ctx.rank;
+  const size_t hi = (lo + per < a.n4) ? lo + per : a.n4;
+  if (ok && lo < hi) {
+    const size_t e_lo = 4 * lo, e_hi = 4 * hi;
+    if (a.K <= 2) robust_body<2, 1>(ctx, a, e_lo, e_hi);
+    else if (a.K <= 4) robust_body<4, 2>(ctx, a, e_lo, e_hi);
+    else if (a.K <= 8) robust_body<8, 3>(ctx, a, e_lo, e_hi);
+    else if (a.K <= 16) robust_body<16, 4>(ctx, a, e_lo, e_hi);
+    else robust_body<32, 5>(ctx, a, e_lo, e_hi);
+  }
+  rank_barrier(ctx, e0 + 2);  // all robust slices are in every rank's dst; uploads may be rewritten
+  block_epoch_end(ctx, e0 + 2);
 }
 
 // ----------------------------------------------------------------------------- C4
@@ -621,6 +755,28 @@ int flpr_comm_reduce_bcast_nvls(int rank, int world, void* const* flag_pages, do
 }
 
 void flpr_comm_set_one_shot_bytes(int bytes) { g_one_shot_bytes = bytes; }
+
+// Robust aggregate of K uploads into every rank's `dst`: rule 0 = coordinate-wise median, 1 = trimmed mean of sorted
+// positions [b, K - b). Returns -1 (K or world out of range), -2 (n % 4), -3 (unknown rule, or b outside [0, K/2) for
+// the trimmed mean / not 0 for the median).
+int flpr_comm_reduce_robust(int rank, int world, void* const* flag_pages, double timeout_s, int K,
+                            const float* const* src, float* const* dst, int rule, int b, size_t n, int nblocks,
+                            cudaStream_t st) {
+  if (K < 1 || K > MAX_CLIENTS || world < 1 || world > MAX_RANKS) return -1;
+  if (n % 4) return -2;
+  if (rule == ROBUST_MEDIAN ? b != 0 : (rule != ROBUST_TRIMMED_MEAN || b < 0 || 2 * b >= K)) return -3;
+  CommCtx c = make_ctx(rank, world, flag_pages, timeout_s);
+  RobustArgs a;
+  memset(&a, 0, sizeof(a));
+  a.K = K;
+  a.rule = rule;
+  a.b = b;
+  for (int i = 0; i < K; ++i) a.src[i] = src[i];
+  for (int r = 0; r < world; ++r) a.dst[r] = dst[r];
+  a.n4 = n / 4;
+  fed_reduce_robust_kernel<<<clamp_blocks(nblocks), COMM_THREADS, 0, st>>>(c, a);
+  return (int)cudaGetLastError();
+}
 
 int flpr_comm_mix(int rank, int world, void* const* flag_pages, double timeout_s, int K, int L,
                   const float* const* src, const float* w_rows /* host [L*K] or null */,

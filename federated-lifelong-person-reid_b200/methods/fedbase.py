@@ -14,6 +14,7 @@ The dict payloads of the reference protocol are still produced (as named views) 
 """
 from __future__ import annotations
 
+import math
 from typing import Any, Dict, List, Optional
 
 import torch
@@ -167,23 +168,61 @@ def parse_server_opt(cfg: Optional[Dict]) -> Optional[Dict[str, Any]]:
     return out
 
 
+def parse_aggregator(cfg: Optional[Dict]) -> Optional[Dict[str, Any]]:
+    """Validate the ``server: aggregator:`` block, ``{name: median}`` or ``{name: trimmed_mean, beta: 0.2}``, and return
+    it with the default ``beta`` (0.1) filled in (``None``: no block, the ``train_cnt``-weighted mean). ``beta`` must be
+    a finite number with ``0 <= beta < 0.5``. Raises ``ValueError`` on an unknown name or key or a bad ``beta``."""
+    if cfg is None:
+        return None
+    if not isinstance(cfg, dict):
+        raise ValueError(f"aggregator must be a mapping, got {cfg!r}")
+    name = cfg.get("name")
+    allowed = {"median": set(), "trimmed_mean": {"beta"}}
+    if name not in allowed:
+        raise ValueError(f"aggregator: unknown name {name!r} (one of {sorted(allowed)})")
+    unknown = sorted(set(cfg) - allowed[name] - {"name"})
+    if unknown:
+        raise ValueError(f"aggregator: unknown key(s) {unknown} for {name!r} (allowed: {sorted(allowed[name])})")
+    if name == "median":
+        return {"name": name}
+    beta = cfg.get("beta", 0.1)
+    if isinstance(beta, bool) or not isinstance(beta, (int, float)):
+        raise ValueError(f"aggregator: beta must be a number, got {beta!r}")
+    beta = float(beta)
+    if not (math.isfinite(beta) and 0 <= beta < 0.5):
+        raise ValueError(f"aggregator: beta must be finite and in [0, 0.5), got {beta}")
+    return {"name": name, "beta": beta}
+
+
+def trim_count(beta: float, K: int) -> int:
+    """Values cut from each end by ``trimmed_mean`` over ``K`` uploads: ``floor(beta * K)``, the cut of
+    ``scipy.stats.trim_mean``."""
+    return int(beta * K)
+
+
 class FedServer(ServerModule):
     """Server role of the FedAvg-family exchange (replicated on every rank).
 
     ``server_opt`` (optional, :func:`parse_server_opt`): instead of overwriting the replica with the aggregated mean,
     ``calculate()`` takes one server-optimizer step toward it (FedAvgM / FedAdagrad / FedAdam / FedYogi,
     ``ops.fused.server_opt_step``). ``glob`` is bitwise identical on every rank, so the replicated step keeps the replicas
-    (and their moments ``m`` / ``v``) identical without any extra communication."""
+    (and their moments ``m`` / ``v``) identical without any extra communication.
+
+    ``aggregator`` (optional, :func:`parse_aggregator`): ``glob`` is the coordinate-wise median or trimmed mean of the
+    uploads (unweighted, ``FedComm.reduce_robust``) instead of their ``train_cnt``-weighted mean. It has no state, and
+    ``server_opt`` steps toward it like toward the mean."""
 
     upload_key = "incremental_model_params"
     integrated_key = "integrated_model_params"
     payload_prefix = "net."
 
-    def __init__(self, server_name, model, operator, ckpt_root, server_opt: Optional[Dict] = None, **kwargs):
+    def __init__(self, server_name, model, operator, ckpt_root, server_opt: Optional[Dict] = None,
+                 aggregator: Optional[Dict] = None, **kwargs):
         super().__init__(server_name, model, operator, ckpt_root, **kwargs)
         self.client_ids: Dict[str, int] = {}
         self.uploaded: List[int] = []                       # client ids with a valid upload slot (insertion order)
         self.server_opt = parse_server_opt(server_opt)
+        self.aggregator = parse_aggregator(aggregator)
         self.opt_m: Optional[torch.Tensor] = None           # server-optimizer moments, fp32, allocated on first use
         self.opt_v: Optional[torch.Tensor] = None
 
@@ -206,6 +245,11 @@ class FedServer(ServerModule):
     def aggregate(self) -> Optional[torch.Tensor]:
         if not self.uploaded:
             return None
+        agg = self.aggregator
+        if agg is not None:
+            b = trim_count(agg["beta"], len(self.uploaded)) if agg["name"] == "trimmed_mean" else 0
+            self.comm.reduce_robust("up", "glob", self.uploaded, agg["name"], b)
+            return self.comm.rank_view("glob")
         self.comm.reduce_bcast("up", "glob", self.uploaded, cnt="cnt")
         return self.comm.rank_view("glob")
 

@@ -51,6 +51,7 @@ def _signatures() -> dict:
         "flpr_comm_barrier": [I, I, P, D, P],
         "flpr_comm_reduce_bcast": [I, I, P, D, I, P, P, P, P, Z, I, P],
         "flpr_comm_reduce_bcast_nvls": [I, I, P, D, I, P, P, P, I, P, F, P, P, P, Z, I, P],
+        "flpr_comm_reduce_robust": [I, I, P, D, I, P, P, I, I, Z, I, P],
         "flpr_comm_set_channel": [I],
         "flpr_comm_mix": [I, I, P, D, I, I, P, P, P, P, P, P, Z, I, P],
         "flpr_comm_curv_moments": [I, I, P, D, I, P, P, P, P, P, Z, I, P],

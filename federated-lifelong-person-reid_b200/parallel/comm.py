@@ -49,6 +49,21 @@ def _dist_ready() -> bool:
     return dist.is_available() and dist.is_initialized()
 
 
+def robust_aggregate(stack: torch.Tensor, rule: str, b: int = 0) -> torch.Tensor:
+    """Coordinate-wise ``median`` / ``trimmed_mean`` of ``stack`` ``[K, n]`` (fp32) over its client dimension, with the
+    ordering and arithmetic of ``fed_reduce_robust_kernel`` (see ``FedComm.reduce_robust``)."""
+    K = stack.shape[0]
+    s = torch.sort(stack, dim=0, stable=True).values
+    if rule == "median":
+        if K % 2:
+            return s[(K - 1) // 2].clone()
+        return s[K // 2 - 1] * 0.5 + s[K // 2] * 0.5
+    acc = torch.full_like(s[0], -0.0)                 # (-0.0 is the exact identity of the addition)
+    for t in range(b, K - b):
+        acc = acc + s[t]
+    return acc / torch.full_like(acc, float(K - 2 * b))  # (a true division, also on CUDA)
+
+
 class FedComm:
     def __init__(self, device: torch.device | str, num_clients: int, arena_bytes: int = 1 << 30,
                  mode: Optional[str] = None, timeout_s: float = 30.0, comm_blocks: int = 0, group=None):
@@ -329,6 +344,36 @@ class FedComm:
         else:
             w = torch.tensor(list(weights), dtype=torch.float32, device=stack.device)
         self.rank_view(dst).copy_((w[:, None] * stack).sum(0))
+
+    ROBUST_RULES = ("median", "trimmed_mean")       # index = the ``rule`` code of ``flpr_comm_reduce_robust``
+
+    def reduce_robust(self, src: str, dst: str, clients: Sequence[int], rule: str, b: int = 0) -> None:
+        """C1+C2, Byzantine-robust: ``dst`` = coordinate-wise ``median`` or ``trimmed_mean`` of the uploads of ``clients``
+        on every rank, unweighted. Per coordinate the K values are ordered by ``(value, position in clients)`` (NaN
+        above +inf, -0.0 == +0.0), i.e. a stable sort. ``median``: the middle value, or ``0.5 * lo + 0.5 * hi`` of the
+        two middle values for even K. ``trimmed_mean``: the mean of sorted positions ``[b, K - b)``, summed in fp32 in
+        ascending order. ``p2p`` runs ``fed_reduce_robust_kernel`` (two-shot; never the NVLS path, whose in-switch sums
+        cannot form order statistics); the other modes all-gather and sort."""
+        bs, bd = self.bufs[src], self.bufs[dst]
+        assert bs.n == bd.n and bs.dtype == torch.float32 and bd.dtype == torch.float32
+        if rule not in self.ROBUST_RULES:
+            raise ValueError(f"reduce_robust: unknown rule {rule!r} (one of {self.ROBUST_RULES})")
+        K, b = len(clients), int(b)
+        if not (b == 0 if rule == "median" else 0 <= 2 * b < K):
+            raise ValueError(f"reduce_robust: b = {b} out of range for {rule!r} with {K} clients")
+        if self.mode == "p2p":
+            rc = self._lib.flpr_comm_reduce_robust(self.rank, self.world, self._flag_pages, self.timeout_s, K,
+                                                   self._client_ptrs(src, clients), self._rank_ptrs(dst),
+                                                   self.ROBUST_RULES.index(rule), b, bs.n,
+                                                   self._grid_for(bs.n * 4 * max(K, 1) // max(self.world, 1)),
+                                                   self._stream())
+            native.check(rc, "flpr_comm_reduce_robust")
+            native.count_launch()
+            self.poll_errors()
+            share = bs.n * 4 / self.world
+            self.bytes_moved += int(share * self._remote(clients) + share * (self.world - 1))
+            return
+        self.rank_view(dst).copy_(robust_aggregate(self._gather_clients(src, clients).float(), rule, b))
 
     def _reduce_bcast_nvls(self, src, dst, clients, mine, cnt, weights) -> None:
         """C1+C2 through the switch: local fold of this rank's clients -> ``multimem.ld_reduce`` of the partials for

@@ -110,11 +110,12 @@ def _operator(exp_config: Dict, model: ModelModule):
 def parser_server(exp_config: Dict, common_config: Dict, device="cpu", store: Optional[CheckpointStore] = None,
                   comm=None) -> ServerModule:
     method = exp_config["exp_method"]
-    if "server_opt" in exp_config["server"]:
-        from ..methods.fedbase import FedServer
-        if not issubclass(methods[method].Server, FedServer):
-            # every other server role has its own aggregation (or none): the key would otherwise be dropped silently
-            raise ValueError(f"server.server_opt is only supported by fedavg, fedprox and fedcurv, not by {method!r}")
+    for key in ("server_opt", "aggregator"):
+        if key in exp_config["server"]:
+            from ..methods.fedbase import FedServer
+            if not issubclass(methods[method].Server, FedServer):
+                # every other server role has its own aggregation (or none): the key would otherwise be dropped silently
+                raise ValueError(f"server.{key} is only supported by fedavg, fedprox and fedcurv, not by {method!r}")
     eng = dict(exp_config.get("engine_opts", {}), num_clients=len(exp_config["clients"]))
     model = parser_model(exp_config["exp_method"], exp_config["model_opts"], device, eng,
                          exp_config["server"]["server_name"])
